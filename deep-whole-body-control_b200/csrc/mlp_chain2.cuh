@@ -2,17 +2,20 @@
 //
 //   * A CTA works on one or two 128-row tiles (slots X and Y).  Each slot owns ONE operand tile in shared memory that every op updates
 //     in place: two warpgroups multiply the tile with the op's weight image (64 rows each), run the op's epilogue on their accumulator
-//     fragments and write the result back into the tile as the next op's operand.  A ninth warp streams the weight images in with bulk
-//     copies, the image of op i+1 behind the epilogue of op i.
-//     The wgmmas of an op are issued and awaited by the warps that run its epilogue: nothing of the tensor-core work overlaps that
-//     epilogue, and ptxas reports (C7520) that it serialises the wgmma instructions of this kernel.  What that costs is not measured.
+//     fragments and write the result back into the tile as the next op's operand.  A third warpgroup gives its registers to the workers
+//     (setmaxnreg 40 / 232); its first warp streams the weight images in with bulk copies, the image of op i+1 behind the epilogue of op i.
+//     All wgmmas of an op form one pipeline: one wait per op, not per instruction.  ptxas silently falls back to fencing and awaiting
+//     every wgmma when the control flow around them does not look warp-uniform to it (C7520), which values loaded from shared memory (the
+//     queue item, the program's fields) do not: those pass through c2_uni.  The wgmmas of an op are still issued and awaited by the warps
+//     that run its epilogue, so nothing of the tensor-core work overlaps that epilogue.  The workers use all 232 registers and spill the
+//     prefetched activation chunks of the backward epilogue (x) to local memory around the 3xTF32 wgmmas.
 //   * Both slots run the same program, so one weight image per op serves two tiles (half the L2 traffic per tile).
 //   * The trunk a second head needs is re-read from the activation buffer the backward pass needs anyway (L2 hit) instead
 //     of occupying a second shared-memory tile.
 //   * "3xTF32" (precision 2): x = hi + lo with hi = the 19 leading bits the tensor core reads (it TRUNCATES the 13 low mantissa bits
 //     of a 32-bit operand) and lo = x - hi (exact in fp32).  D = A_hi W_hi + A_lo W_hi + A_hi W_lo: the first and third products read the
 //     fp32 tile / the raw and the "lo" weight image from shared memory, the second takes A_lo as a register operand, formed by each
-//     thread from its A fragment.  The dropped A_lo W_lo term is 2^-22 relative: fp32-grade results.  The "lo" image occupies the second
+//     thread from its A fragment for the whole op before / while its wgmmas run (c2_mma_op).  The dropped A_lo W_lo term is 2^-22 relative: fp32-grade results.  The "lo" image occupies the second
 //     slot's tile, so 3xTF32 items hold one tile.
 //   * The heads' epilogues finish the job (north_star: "log-prob, ratio/clip/min and entropy fused into the epilogue"):
 //     rollout: action sampling + two-channel Gaussian log-prob (AC:326-345); update: PPO surrogate / clipped value loss /
@@ -37,7 +40,9 @@ constexpr int C2_TILE = 128 * 128;                       // floats per operand t
 constexpr int C2_WORKERS = 8;                            // load / wgmma / epilogue warps: two warpgroups, warp w owns tile rows [16 w, 16 w + 16)
 constexpr int C2_H = 2;                                  // column groups of the epilogue: half-warp h takes the 32-column chunks h and h + 2
 constexpr int C2_CPW = 4 / C2_H;                         // chunks per thread and op (N <= 128)
-constexpr int C2_THREADS = 32 * (C2_WORKERS + 1);        // + the weight-copy warp (warp 8)
+constexpr int C2_THREADS = 32 * (C2_WORKERS + 4);        // + a third warpgroup whose first warp (warp 8) copies the weight images
+constexpr int C2_REGS_WORKER = 232, C2_REGS_COPY = 40;   // setmaxnreg: 256 x 232 + 128 x 40 = 64 512 of the SM's 65 536 registers
+constexpr int C2_KSET = TC_MAXK / 16;                    // 3xTF32: K steps per set of A_lo fragment registers (two sets cover kpad <= 128)
 constexpr int C2_NW = 32 * C2_WORKERS;                   // 256 worker threads
 constexpr int C2_SMEM_FLOATS = 3 * C2_TILE + 2 * 128 + C2_WORKERS * 1024;    // tile X, tile Y, weight image, two bias slots, transposition buffers
 
@@ -177,6 +182,11 @@ __device__ __forceinline__ bool c2_elect() {
       : "=r"(pred));
   return pred != 0;
 }
+// a value every lane of the (converged) warp holds, in a form the compiler can see is warp-uniform: control flow around wgmma that depends
+// on shared-memory loads is "divergent" to ptxas, which then fences and awaits every wgmma on its own (C7520)
+__device__ __forceinline__ int c2_uni(int v) { return __shfl_sync(0xffffffffu, v, 0); }
+template <int kRegs> __device__ __forceinline__ void c2_reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+template <int kRegs> __device__ __forceinline__ void c2_reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs)); }
 __device__ __forceinline__ void c2_wbar() { __syncwarp(); asm volatile("bar.sync 1, %0;" ::"n"(C2_NW) : "memory"); }     // the worker warps
 constexpr float C2_LOG_SQRT_2PI = 0.91893853320467274178f;
 
@@ -422,19 +432,34 @@ __device__ __forceinline__ void c2_mma_op(float (&acc)[64], uint32_t a0, uint32_
     for (int k = 0; k < nk; ++k, ad += 16, bd += 16) wg_mma_ss<N>(acc, ad, bd, k > 0);
   } else {
     // D = A_hi W_hi + A_lo W_hi + A_hi W_lo: the tensor core truncates the fp32 tile and the raw image to their high parts itself; A_lo is
-    // formed in registers (the A fragment of this thread) and fed as a register operand.  One K step per commit group: the four fragment
-    // registers are rewritten only after the group that read them has retired.
-    uint64_t bl = tc_desc(b0_lo, 128, wsbo);
-    for (int k = 0; k < nk; ++k, ad += 16, bd += 16, bl += 16) {
-      const float* ap = arow + (size_t)k * 64;           // 8 columns = two pieces of 32 floats
-      const uint32_t l0 = __float_as_uint(tf32_lo(ap[0])), l1 = __float_as_uint(tf32_lo(ap[1024]));          // rows +0 / +8 (next 8-row group)
-      const uint32_t l2 = __float_as_uint(tf32_lo(ap[32])), l3 = __float_as_uint(tf32_lo(ap[1024 + 32]));    // columns +4
+    // formed in registers (the A fragment of this thread) and fed as a register operand.  The fragments of a whole op (16 K steps x 4
+    // registers) stay live until the op's single wait, in two sets of C2_KSET K steps with a commit group each: the second set is formed
+    // while the wgmmas of the first execute, and nothing is awaited inside the op.  (Two smaller sets recycled behind wait<1> made ptxas
+    // serialise the wgmmas again: C7511, not enough registers for the pipeline.)
+    // Per accumulator the products keep the order hi*hi, lo*hi, hi*lo per K step, K ascending.
+    const uint64_t bl = tc_desc(b0_lo, 128, wsbo);
+    uint32_t lo[2][C2_KSET][4];
+#pragma unroll
+    for (int g = 0; g < 2; ++g) {
+#pragma unroll
+      for (int j = 0; j < C2_KSET; ++j) {
+        if (C2_KSET * g + j < nk) {
+          const float* ap = arow + (size_t)(C2_KSET * g + j) * 64;          // 8 columns = two pieces of 32 floats
+          lo[g & 1][j][0] = __float_as_uint(tf32_lo(ap[0])); lo[g & 1][j][1] = __float_as_uint(tf32_lo(ap[1024]));          // rows +0 / +8 (next 8-row group)
+          lo[g & 1][j][2] = __float_as_uint(tf32_lo(ap[32])); lo[g & 1][j][3] = __float_as_uint(tf32_lo(ap[1024 + 32]));    // columns +4
+        }
+      }
       wg_fence();
-      wg_mma_ss<N>(acc, ad, bd, k > 0);
-      wg_mma_rs<N>(acc, l0, l1, l2, l3, bd, 1);
-      wg_mma_ss<N>(acc, ad, bl, 1);
+#pragma unroll
+      for (int j = 0; j < C2_KSET; ++j) {
+        const int k = C2_KSET * g + j;
+        if (k < nk) {
+          wg_mma_ss<N>(acc, ad + 16 * k, bd + 16 * k, k > 0);
+          wg_mma_rs<N>(acc, lo[g & 1][j][0], lo[g & 1][j][1], lo[g & 1][j][2], lo[g & 1][j][3], bd + 16 * k, 1);
+          wg_mma_ss<N>(acc, ad + 16 * k, bl + 16 * k, 1);
+        }
+      }
       wg_commit();
-      wg_wait<0>();
     }
   }
   wg_commit();
@@ -449,11 +474,11 @@ __global__ void __launch_bounds__(C2_THREADS, 1) chain2_kernel(const __grid_cons
   __shared__ C2Shared sh;
   __shared__ __align__(16) C2Prog sprog;
   int cur_prog = -1;
-  float* tile[2] = {c2_smem, c2_smem + C2_TILE};
+  auto tile = [&](int s) { return c2_smem + s * C2_TILE; };      // operand tile of slot s
   float* wbuf = c2_smem + 2 * C2_TILE;
   float* bias_s = c2_smem + 3 * C2_TILE;                 // two slots of 128 (parity of the CTA-wide op counter)
   float* stage_s = bias_s + 2 * 128;                     // per worker warp: [16 rows][64 columns] transposition buffer of the epilogue
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31, warp = c2_uni(tid >> 5);
   if (tid == 0) {
     tc_mbar_init(&sh.w_full, 1);
     tc_mbar_init(&sh.w_free, 1);
@@ -469,60 +494,70 @@ __global__ void __launch_bounds__(C2_THREADS, 1) chain2_kernel(const __grid_cons
   uint32_t nop = 0, nld = 0;
   uint32_t nw = 0, nf = 0;          // weight images consumed (phase of w_full: workers) / released (phase of w_free: copy warp)
 
-  for (;;) {
-    // ---- next work item ----
+  // ---- next work item (every thread of the CTA, workers and copy warpgroup alike): false when the queue is empty ----
+  int t0, nslots;                                        // first tile, tiles of this item
+  auto next_item = [&]() {
     __syncthreads();                                     // everybody is done with the previous item (sh.item may be overwritten)
     if (tid == 0) sh.item = atomicAdd(L.queue, 1);
     __syncthreads();
-    const int item = sh.item;
-    if (item >= items) break;
-    int pi, t0, nslots;                                  // program (0 = the longer one, first), first tile, tiles of this item
-    {
-      const bool two = item < n_pair_items;
-      const int k = two ? item : item - n_pair_items, per = two ? L.np2 : L.ns1;
-      pi = k / per;
-      t0 = two ? 2 * (k - pi * per) : 2 * L.np2 + (k - pi * per);
-      nslots = min(two ? 2 : 1, tiles - t0);
-      asm volatile("" : "+r"(nslots));                   // opaque: one body for both item sizes (the compiler cloned the whole item loop otherwise)
-    }
-    // slot s works on tile tb + s * td: upwards from t0, or (L.rev: the backward launch) downwards from the last tile -- the forward launch
-    // that produced the activation images this one reads walked upwards, so its most recent output, still in L2, belongs to the last tiles
-    const int tb = L.rev ? tiles - 1 - t0 : t0, td = L.rev ? -1 : 1;
+    const int item = c2_uni(sh.item);
+    if (item >= items) return false;
+    const bool two = item < n_pair_items;
+    const int k = two ? item : item - n_pair_items, per = two ? L.np2 : L.ns1;
+    const int pi = k / per;                              // program (0 = the longer one, first)
+    t0 = two ? 2 * (k - pi * per) : 2 * L.np2 + (k - pi * per);
+    nslots = min(two ? 2 : 1, tiles - t0);
+    asm volatile("" : "+r"(nslots));                     // opaque: one body for both item sizes (the compiler cloned the whole item loop otherwise)
+    nslots = c2_uni(nslots);
     // the item's program goes to shared memory: read through the kernel parameter, every field access with a run-time op index is an
     // indexed constant-bank load -- a long-scoreboard stall in front of most addresses and predicates of the epilogue
     if (pi != cur_prog) {
       const int4* src = reinterpret_cast<const int4*>(&L.p[pi]);
       int4* dst = reinterpret_cast<int4*>(&sprog);
-      for (int k = tid; k < (int)(sizeof(C2Prog) / 16); k += C2_THREADS) dst[k] = src[k];
+      for (int k4 = tid; k4 < (int)(sizeof(C2Prog) / 16); k4 += C2_THREADS) dst[k4] = src[k4];
       cur_prog = pi;
       __syncthreads();
     }
-    const C2Prog& pr = sprog;
-    const int nops = pr.n_ops;
+    return true;
+  };
+  const C2Prog& pr = sprog;
 
-    if (warp == C2_WORKERS) {
-      // ===================== weight copies =====================
-      // One image is resident at a time: the image (and bias) of op i+1 is fetched as soon as the workers have retired the wgmmas of op i,
-      // i.e. behind the epilogue of op i.  3xTF32 items hold one tile (launch_chain2n), so the image of the weights' low parts travels with
-      // the raw image into the unused tile of slot 1.
-      auto fetch = [&](const C2Op& o, uint32_t slot) {
-        const uint32_t wbytes = (uint32_t)(o.npad * o.kpad) * 4u, bbytes = (uint32_t)o.npad * 4u;
-        if (c2_elect()) {
-          c2_expect_tx(&sh.w_full, wbytes + bbytes + (x3 ? wbytes : 0u));
-          c2_bulk_g2s(wbuf, o.wp, wbytes, &sh.w_full);
-          c2_bulk_g2s(bias_s + slot * 128, o.wp + (wbytes >> 2), bbytes, &sh.w_full);
-          if (x3) c2_bulk_g2s(tile[1], o.wp_lo, wbytes, &sh.w_full);
+  if (warp >= C2_WORKERS) {
+    // ===================== weight copies (third warpgroup; its warps 9-11 only take part in the CTA-wide barriers) =====================
+    c2_reg_dec<C2_REGS_COPY>();
+    while (next_item()) {
+      const int nops = c2_uni(pr.n_ops);
+      if (warp == C2_WORKERS) {
+        // One image is resident at a time: the image (and bias) of op i+1 is fetched as soon as the workers have retired the wgmmas of op i,
+        // i.e. behind the epilogue of op i.  3xTF32 items hold one tile (launch_chain2n), so the image of the weights' low parts travels with
+        // the raw image into the unused tile of slot 1.
+        auto fetch = [&](const C2Op& o, uint32_t slot) {
+          const uint32_t wbytes = (uint32_t)(o.npad * o.kpad) * 4u, bbytes = (uint32_t)o.npad * 4u;
+          if (c2_elect()) {
+            c2_expect_tx(&sh.w_full, wbytes + bbytes + (x3 ? wbytes : 0u));
+            c2_bulk_g2s(wbuf, o.wp, wbytes, &sh.w_full);
+            c2_bulk_g2s(bias_s + slot * 128, o.wp + (wbytes >> 2), bbytes, &sh.w_full);
+            if (x3) c2_bulk_g2s(tile(1), o.wp_lo, wbytes, &sh.w_full);
+          }
+          __syncwarp();
+        };
+        fetch(pr.op[0], nop & 1);
+        for (int i = 0; i + 1 < nops; ++i) {
+          tc_mbar_wait(&sh.w_free, nf & 1); ++nf;          // every wgmma reading image i has retired: the buffer may be refilled
+          fetch(pr.op[i + 1], (nop + i + 1) & 1);
         }
-        __syncwarp();
-      };
-      fetch(pr.op[0], nop & 1);
-      for (int i = 0; i + 1 < nops; ++i) {
-        tc_mbar_wait(&sh.w_free, nf & 1); ++nf;          // every wgmma reading image i has retired: the buffer may be refilled
-        fetch(pr.op[i + 1], (nop + i + 1) & 1);
+        tc_mbar_wait(&sh.w_free, nf & 1); ++nf;
       }
-      tc_mbar_wait(&sh.w_free, nf & 1); ++nf;
-    } else {
-      // ===================== loads, wgmma and epilogues (two warpgroups) =====================
+      nop += nops;
+    }
+  } else {
+    // ===================== loads, wgmma and epilogues (two warpgroups) =====================
+    c2_reg_inc<C2_REGS_WORKER>();
+    while (next_item()) {
+      const int nops = c2_uni(pr.n_ops);
+      // slot s works on tile tb + s * td: upwards from t0, or (L.rev: the backward launch) downwards from the last tile -- the forward launch
+      // that produced the activation images this one reads walked upwards, so its most recent output, still in L2, belongs to the last tiles
+      const int tb = L.rev ? tiles - 1 - t0 : t0, td = L.rev ? -1 : 1;
       // wgmma: warp w owns tile rows [16 w, 16 w + 16).  Epilogue: the same rows, thread = (row 16 w + lane % 16, 32-column chunks lane / 16
       // and lane / 16 + 2); the accumulator fragments reach that shape through the warp's transposition buffer, 64 columns at a time.
       const int hh = lane >> 4;
@@ -533,7 +568,7 @@ __global__ void __launch_bounds__(C2_THREADS, 1) chain2_kernel(const __grid_cons
 
       // cp.async of one load into the tile of slot s (no waiting); rows beyond the matrix are zero-filled
       auto issue_load = [&](const C2Load& ld, int s, int64_t m0, int rows) {
-        float* tl = tile[s];
+        float* tl = tile(s);
         const int c40 = ld.col0 >> 2, cpr = ld.ncols >> 2;
         const int z0 = (ld.col0 + ld.ncols) >> 2, z1 = ld.zero_to >> 2;
         float* rowbase = tl + ((size_t)(lrow >> 3) * 32) * 32 + (lrow & 7) * 4;
@@ -565,7 +600,7 @@ __global__ void __launch_bounds__(C2_THREADS, 1) chain2_kernel(const __grid_cons
             c2_expect_tx(&sh.ld_bar, (uint32_t)nimg * C2_TILE * 4u);
             for (int s = 0; s < nslots; ++s)
               for (int l = 0; l < pr.n_loads; ++l)
-                if (pr.ld[l].before_op == before && pr.ld[l].img) c2_bulk_g2s(tile[s], pr.ld[l].src.p + (size_t)(tb + s * td) * C2_TILE, C2_TILE * 4, &sh.ld_bar);
+                if (pr.ld[l].before_op == before && pr.ld[l].img) c2_bulk_g2s(tile(s), pr.ld[l].src.p + (size_t)(tb + s * td) * C2_TILE, C2_TILE * 4, &sh.ld_bar);
           }
           tc_mbar_wait(&sh.ld_bar, nld & 1);
           ++nld;
@@ -601,7 +636,7 @@ __global__ void __launch_bounds__(C2_THREADS, 1) chain2_kernel(const __grid_cons
         // the previous op left a finished tile behind: if its output is a tile image it goes out now, as one 64 KB bulk copy issued right
         // before the wgmmas that read the same tile; it must have read the tile before the epilogue of THIS op may overwrite it
         const bool st_prev = i > 0 && pr.op[i - 1].y_img != 0;
-        const int nwid = wg_width(o.npad), nk = o.kpad >> 3;
+        const int nwid = c2_uni(wg_width(o.npad)), nk = c2_uni(o.kpad >> 3);     // (the control flow around the wgmmas)
         for (int s = 0; s < nslots; ++s) {
           const int64_t m0 = (int64_t)(tb + s * td) * TC_M;
           const int rows = (int)min((int64_t)TC_M, (int64_t)pr.M - m0);
@@ -626,14 +661,14 @@ __global__ void __launch_bounds__(C2_THREADS, 1) chain2_kernel(const __grid_cons
             }
           }
           c2_wbar();                                       // the operand tile is complete: loads landed / previous epilogue done (and fenced)
-          if (tid == 0 && st_prev) c2_bulk_s2g(pr.op[i - 1].y + (size_t)(tb + s * td) * C2_TILE, tile[s], C2_TILE * 4);
+          if (tid == 0 && st_prev) c2_bulk_s2g(pr.op[i - 1].y + (size_t)(tb + s * td) * C2_TILE, tile(s), C2_TILE * 4);
           if (s == 0) { tc_mbar_wait(&sh.w_full, nw & 1); ++nw; }
           float acc[64];
           {
-            const uint32_t a0 = tc_smem_u32(tile[s]) + (uint32_t)(warp >> 2) * 8u * 4096u + (uint32_t)(o.a_col0 >> 2) * 128u;
-            const uint32_t b0 = tc_smem_u32(wbuf), b0_lo = tc_smem_u32(tile[1]), wsbo = (uint32_t)(o.kpad >> 2) * 128u;
+            const uint32_t a0 = tc_smem_u32(tile(s)) + (uint32_t)(warp >> 2) * 8u * 4096u + (uint32_t)(o.a_col0 >> 2) * 128u;
+            const uint32_t b0 = tc_smem_u32(wbuf), b0_lo = tc_smem_u32(tile(1)), wsbo = (uint32_t)(o.kpad >> 2) * 128u;
             // A fragment element (row 16 warp + lane / 4, column a_col0 + lane % 4) of this thread
-            const float* arow = tile[s] + ((size_t)(2 * warp) * 32 + (o.a_col0 >> 2)) * 32 + (lane >> 2) * 4 + (lane & 3);
+            const float* arow = tile(s) + ((size_t)(2 * warp) * 32 + (o.a_col0 >> 2)) * 32 + (lane >> 2) * 4 + (lane & 3);
             if (nwid == 32) c2_mma_op<32>(acc, a0, b0, b0_lo, wsbo, nk, x3, arow);
             else if (nwid == 64) c2_mma_op<64>(acc, a0, b0, b0_lo, wsbo, nk, x3, arow);
             else c2_mma_op<128>(acc, a0, b0, b0_lo, wsbo, nk, x3, arow);
@@ -692,7 +727,7 @@ __global__ void __launch_bounds__(C2_THREADS, 1) chain2_kernel(const __grid_cons
                 }
               }
               if (o.out_col0 >= 0) {
-                float* otile = tile[s] + ((size_t)((r >> 3) * 32 + ((o.out_col0 + c0) >> 2)) * 8 + (r & 7)) * 4;
+                float* otile = tile(s) + ((size_t)((r >> 3) * 32 + ((o.out_col0 + c0) >> 2)) * 8 + (r & 7)) * 4;
 #pragma unroll
                 for (int j4 = 0; j4 < 8; ++j4)
                   *reinterpret_cast<float4*>(otile + (size_t)j4 * 32) = make_float4(v[4 * j4], v[4 * j4 + 1], v[4 * j4 + 2], v[4 * j4 + 3]);
@@ -729,12 +764,12 @@ __global__ void __launch_bounds__(C2_THREADS, 1) chain2_kernel(const __grid_cons
       if (pr.op[nops - 1].y_img) {
         c2_wbar();
         if (tid == 0) {
-          for (int s = 0; s < nslots; ++s) c2_bulk_s2g(pr.op[nops - 1].y + (size_t)(tb + s * td) * C2_TILE, tile[s], C2_TILE * 4);
+          for (int s = 0; s < nslots; ++s) c2_bulk_s2g(pr.op[nops - 1].y + (size_t)(tb + s * td) * C2_TILE, tile(s), C2_TILE * 4);
           c2_bulk_wait_read();
         }
       }
+      nop += nops;
     }
-    nop += nops;
   }
   if (tid == 0) c2_bulk_wait_all();      // the image stores of this CTA have landed
   __syncthreads();
