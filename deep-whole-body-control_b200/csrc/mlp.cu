@@ -703,6 +703,51 @@ static int build_backward(const DwbcNetCfg& n, const float* P, const Plan& p, C2
   return DWBC_OK;
 }
 
+// The chain programs of one entry point and the pack list of their weight images.  b[] = {A, C, A2, C2} for dwbc_policy_act, {C, C2} for
+// dwbc_critic_values, {A, C, Ab, Cb} (forward + loss, backward) for dwbc_ppo_minibatch_grad.  The builders point at pl / off: never copied.
+struct C2Chains {
+  C2PackList pl{};
+  int64_t off = 0;
+  C2Builder b[4];
+  int nprog = 0;
+  C2Chains(float* wpack, int rows, bool x3)
+      : b{C2Builder(&pl, &off, rows, x3), C2Builder(&pl, &off, rows, x3), C2Builder(&pl, &off, rows, x3), C2Builder(&pl, &off, rows, x3)} {
+    pl.out = wpack;
+  }
+  C2Chains(const C2Chains&) = delete;
+  C2Chains& operator=(const C2Chains&) = delete;
+};
+
+// THE decision between the fused chains and the layer-wise path, for every entry point: builds all programs the call would launch (host
+// code only: nothing is packed or launched) and returns true when the network fits the tile layout (chain_usable) AND every builder
+// accepted its ops and loads AND the weight images of all programs fit one pack list (C2_MAX_OPS, C2_MAX_LOADS, C2_MAX_PACK,
+// C2_PACK_FLOATS).  A network that passes chain_usable can still fail the latter (e.g. three 128-wide backbone layers per network: 38
+// images in the update); it then runs layer-wise like any network with a layer wider than 128.
+// what: 0 = dwbc_policy_act (`hist`: the latent comes from the history encoder, in p.zh), 1 = dwbc_critic_values, 2 =
+// dwbc_ppo_minibatch_grad (`idx`: its gather index).  `sms`: the SM count the rollout's split into one program per head follows.
+static bool plan_chains(C2Chains& c, int what, const DwbcNetCfg& n, const float* P, const float* obs, const int64_t* idx, int64_t obs_stride,
+                        bool hist, float* values, const Plan& p, int rows, int sms) {
+  if (!chain_usable(n, p, obs, obs_stride)) return false;
+  const int tiles = (rows + TC_M - 1) / TC_M, zld = (int)align_up(p.latent, 4);
+  C2Builder* B = c.b;
+  int rc;
+  if (what == 0) {
+    const bool split = 4 * tiles <= sms;       // few tiles (the rollout): one program per HEAD, four short programs spread over 4 x tiles SMs
+    rc = build_forward(n, P, obs, nullptr, obs_stride, hist ? p.zh : nullptr, zld, p, values, false, 1, &B[0], &B[1], split ? &B[2] : nullptr,
+                       split ? &B[3] : nullptr);
+    c.nprog = split ? 4 : 2;
+  } else if (what == 1) {
+    const bool split = 2 * tiles <= sms;
+    rc = build_forward(n, P, obs, nullptr, obs_stride, nullptr, 0, p, values, false, 0, nullptr, &B[0], nullptr, split ? &B[1] : nullptr);
+    c.nprog = split ? 2 : 1;
+  } else {
+    rc = build_forward(n, P, obs, idx, obs_stride, nullptr, zld, p, values, true, 2, &B[0], &B[1]);
+    if (rc == DWBC_OK) rc = build_backward(n, P, p, B[2], B[3]);
+    c.nprog = 2;
+  }
+  return rc == DWBC_OK && c.off <= C2_PACK_FLOATS;
+}
+
 // every layer's weight gradient of both networks in one persistent launch (wgrad_group.cuh)
 static int weight_gradients(const DwbcNetCfg& n, float* grad, const DwbcStorage* s, const int64_t* idx, int rows, const Plan& p, cudaStream_t st) {
   const int Lld = (int)align_up(p.latent, 4);
@@ -764,21 +809,13 @@ extern "C" int dwbc_policy_act(const DwbcNetCfg* net, const float* params, const
   Plan p = make_plan(n, rows, workspace);
   const float* z;
   int zld = (int)align_up(p.latent, 4);
-  if (chain_usable(n, p, obs, obs_stride)) {
+  const bool x3 = mlp_precision == 2;
+  C2Chains ch(p.wpack, rows, x3);
+  if (plan_chains(ch, 0, n, params, obs, nullptr, obs_stride, hist_encoding != 0, values, p, rows, c2_sm_count())) {
     if (hist_encoding) TRY(hist_latent_only(n, params, obs, nullptr, obs_stride, rows, p, p.zh, zld, st));
-    C2PackList pl{};
-    pl.out = p.wpack;
-    int64_t off = 0;
-    const bool x3 = mlp_precision == 2;
-    C2Builder A(&pl, &off, rows, x3), C(&pl, &off, rows, x3), A2(&pl, &off, rows, x3), C2(&pl, &off, rows, x3);
-    // few tiles (the rollout): one program per HEAD, so that four short programs spread over 4 x tiles SMs (build_forward)
-    const bool split = 4 * ((rows + TC_M - 1) / TC_M) <= c2_sm_count();
-    TRY(build_forward(n, params, obs, nullptr, obs_stride, hist_encoding ? p.zh : nullptr, zld, p, values, false, 1, &A, &C, split ? &A2 : nullptr,
-                      split ? &C2 : nullptr));
-    if (off > C2_PACK_FLOATS) return DWBC_ERR_UNSUPPORTED;
-    if (!weights_packed) TRY(launch_pack2(pl, st));       // the images stay valid in the workspace until the parameters change
-    const C2Prog* prs[4] = {&A.pr, &C.pr, &A2.pr, &C2.pr};
-    return launch_chain2n(prs, split ? 4 : 2, fin_rollout(n, params, eps, actions, log_prob, mean, sigma, rows), x3, p.queue, st);
+    if (!weights_packed) TRY(launch_pack2(ch.pl, st));       // the images stay valid in the workspace until the parameters change
+    const C2Prog* prs[4] = {&ch.b[0].pr, &ch.b[1].pr, &ch.b[2].pr, &ch.b[3].pr};
+    return launch_chain2n(prs, ch.nprog, fin_rollout(n, params, eps, actions, log_prob, mean, sigma, rows), x3, p.queue, st);
   }
   if (hist_encoding) {
     TRY(hist_forward(n, params, obs, nullptr, obs_stride, rows, p, st));
@@ -801,17 +838,12 @@ extern "C" int dwbc_critic_values(const DwbcNetCfg* net, const float* params, co
   if (!params || !obs || !values || !workspace || rows <= 0) return DWBC_ERR_ARG;
   cudaStream_t st = (cudaStream_t)stream;
   Plan p = make_plan(*net, rows, workspace);
-  if (chain_usable(*net, p, obs, obs_stride)) {
-    C2PackList pl{};
-    pl.out = p.wpack;
-    int64_t off = 0;
-    const bool x3 = mlp_precision == 2;
-    C2Builder C(&pl, &off, rows, x3), C2(&pl, &off, rows, x3);
-    const bool split = 2 * ((rows + TC_M - 1) / TC_M) <= c2_sm_count();
-    TRY(build_forward(*net, params, obs, nullptr, obs_stride, nullptr, 0, p, values, false, 0, nullptr, &C, nullptr, split ? &C2 : nullptr));
-    TRY(launch_pack2(pl, st));                              // (overwrites the images a previous dwbc_policy_act left behind)
-    const C2Prog* prs[2] = {&C.pr, &C2.pr};
-    return launch_chain2n(prs, split ? 2 : 1, FinArgs{}, x3, p.queue, st);
+  const bool x3 = mlp_precision == 2;
+  C2Chains ch(p.wpack, rows, x3);
+  if (plan_chains(ch, 1, *net, params, obs, nullptr, obs_stride, false, values, p, rows, c2_sm_count())) {
+    TRY(launch_pack2(ch.pl, st));                           // (overwrites the images a previous dwbc_policy_act left behind)
+    const C2Prog* prs[2] = {&ch.b[0].pr, &ch.b[1].pr};
+    return launch_chain2n(prs, ch.nprog, FinArgs{}, x3, p.queue, st);
   }
   return critic_forward(*net, params, obs, nullptr, obs_stride, rows, p, values, st);
 }
@@ -839,23 +871,18 @@ extern "C" int dwbc_ppo_minibatch_grad(const DwbcNetCfg* net, const float* param
   Plan p = make_plan(n, rows, workspace);
   const int Lld = (int)align_up(p.latent, 4);
   const int gleg_ld = (int)align_up(n.n_leg, 4), garm_ld = (int)align_up(n.n_arm, 4);
+  // tensor-core path: forward chains with the loss in the heads' epilogues, backward chains, grouped weight gradients.  The weight images
+  // of all four programs are packed by ONE launch (the parameters are constant within a mini-batch).
+  const bool x3 = mlp_precision == 2;
+  C2Chains ch(p.wpack, rows, x3);
+  const bool chains = plan_chains(ch, 2, n, P, s->observations, idx, s->obs_stride, false, p.value, p, rows, 0);
   if (cudaMemsetAsync(grad, 0, sizeof(float) * n.num_params, st) != cudaSuccess) return DWBC_ERR_LAUNCH;
 
   // forward (the reference evaluates the actor 3x and the priv encoder 3x per mini-batch,
   // PPO:166,174,230; identical values, so each is evaluated once here)
   float* z = p.priv[n.n_priv_layers - 1];
   if (!s->hist_latent) TRY(hist_latent_only(n, P, s->observations, idx, s->obs_stride, rows, p, p.zh, Lld, st));           // PPO:175-176 (no grad)
-  if (chain_usable(n, p, s->observations, s->obs_stride)) {
-    // tensor-core path: forward chains with the loss in the heads' epilogues, backward chains, grouped weight gradients.  The
-    // weight images of all four programs are packed by ONE launch (the parameters are constant within a mini-batch).
-    C2PackList pl{};
-    pl.out = p.wpack;
-    int64_t off = 0;
-    const bool x3 = mlp_precision == 2;
-    C2Builder A(&pl, &off, rows, x3), C(&pl, &off, rows, x3), Ab(&pl, &off, rows, x3), Cb(&pl, &off, rows, x3);
-    TRY(build_forward(n, P, s->observations, idx, s->obs_stride, nullptr, Lld, p, p.value, true, 2, &A, &C));
-    TRY(build_backward(n, P, p, Ab, Cb));
-    if (off > C2_PACK_FLOATS) return DWBC_ERR_UNSUPPORTED;
+  if (chains) {
     FinArgs f{};
     f.std = P + n.off_std; f.idx = idx; f.s_actions = s->actions; f.old_logp = s->log_prob; f.old_values = s->values; f.returns = s->returns;
     f.adv = s->advantages;
@@ -867,9 +894,9 @@ extern "C" int dwbc_ppo_minibatch_grad(const DwbcNetCfg* net, const float* param
     f.clipped_value = hp->use_clipped_value_loss;
     f.ts_target = s->target_arm_torques; f.ts_pos = s->current_arm_dof_pos; f.ts_vel = s->current_arm_dof_vel; f.ts_coef = hp->arm_coefs;
     f.ts_w = hp->torque_supervision_weight;
-    TRY(launch_pack2(pl, st));
-    TRY(launch_chain2(&A.pr, &C.pr, f, x3, p.queue, st));
-    TRY(launch_chain2(&Ab.pr, &Cb.pr, FinArgs{}, x3, p.queue, st, c2_bwd_reverse != 0));
+    TRY(launch_pack2(ch.pl, st));
+    TRY(launch_chain2(&ch.b[0].pr, &ch.b[1].pr, f, x3, p.queue, st));
+    TRY(launch_chain2(&ch.b[2].pr, &ch.b[3].pr, FinArgs{}, x3, p.queue, st, c2_bwd_reverse != 0));
     return weight_gradients(n, grad, s, idx, rows, p, st);
   }
   TRY(priv_forward(n, P, s->observations, idx, s->obs_stride, rows, p, st));
@@ -1040,40 +1067,14 @@ extern "C" int dwbc_debug_describe_chain(const DwbcNetCfg* net, int32_t rows, in
   const float* const obs = reinterpret_cast<const float*>(uintptr_t(3) << 40);
   const int64_t* const idx = what >= 2 ? reinterpret_cast<const int64_t*>(uintptr_t(4) << 40) : nullptr;
   Plan p = make_plan(n, rows, ws);
-  if (!chain_usable(n, p, obs, n.num_obs)) return DWBC_ERR_UNSUPPORTED;
-  C2PackList pl{};
-  pl.out = p.wpack;
-  int64_t off = 0;
-  const bool x3 = mlp_precision == 2;
-  C2Builder A(&pl, &off, rows, x3), C(&pl, &off, rows, x3), A2(&pl, &off, rows, x3), C2(&pl, &off, rows, x3);
-  const C2Prog* prs[4] = {nullptr, nullptr, nullptr, nullptr};
-  int nprog = 0;
-  const int tiles = (rows + TC_M - 1) / TC_M, zld = (int)align_up(p.latent, 4);
-  if (what == 0) {
-    const bool split = 4 * tiles <= sms;
-    TRY(build_forward(n, P, obs, nullptr, n.num_obs, hist_encoding ? p.zh : nullptr, zld, p, p.value, false, 1, &A, &C, split ? &A2 : nullptr, split ? &C2 : nullptr));
-    prs[0] = &A.pr; prs[1] = &C.pr; prs[2] = &A2.pr; prs[3] = &C2.pr;
-    nprog = split ? 4 : 2;
-  } else if (what == 1) {
-    const bool split = 2 * tiles <= sms;
-    TRY(build_forward(n, P, obs, nullptr, n.num_obs, nullptr, 0, p, p.value, false, 0, nullptr, &C, nullptr, split ? &C2 : nullptr));
-    prs[0] = &C.pr; prs[1] = &C2.pr;
-    nprog = split ? 2 : 1;
-  } else {
-    C2Builder Ab(&pl, &off, rows, x3), Cb(&pl, &off, rows, x3);
-    TRY(build_forward(n, P, obs, idx, n.num_obs, nullptr, zld, p, p.value, true, 2, &A, &C));
-    TRY(build_backward(n, P, p, Ab, Cb));
-    static C2Prog keep[2];                 // (the builders of this branch go out of scope)
-    keep[0] = what == 2 ? A.pr : Ab.pr; keep[1] = what == 2 ? C.pr : Cb.pr;
-    prs[0] = &keep[0]; prs[1] = &keep[1];
-    nprog = 2;
-  }
-  if (off > C2_PACK_FLOATS) return DWBC_ERR_UNSUPPORTED;
+  C2Chains ch(p.wpack, rows, mlp_precision == 2);
+  if (!plan_chains(ch, what < 2 ? what : 2, n, P, obs, idx, n.num_obs, hist_encoding != 0, p.value, p, rows, sms)) return DWBC_ERR_UNSUPPORTED;
+  const C2Builder* prs = what == 3 ? ch.b + 2 : ch.b;
   int k = 0;
   auto put = [&](int v) { if (k < out_len) out[k] = v; ++k; };
-  put(nprog); put(pl.n);
-  for (int q = 0; q < nprog; ++q) {
-    const C2Prog& pr = *prs[q];
+  put(ch.nprog); put(ch.pl.n);
+  for (int q = 0; q < ch.nprog; ++q) {
+    const C2Prog& pr = prs[q].pr;
     put(pr.n_ops); put(pr.n_loads);
     for (int i = 0; i < pr.n_ops; ++i) {
       const C2Op& o = pr.op[i];
