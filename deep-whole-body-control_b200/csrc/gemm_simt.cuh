@@ -14,7 +14,41 @@
 
 namespace dwbc {
 
-enum { ACT_NONE = 0, ACT_ELU = 1, ACT_TANH = 2 };
+// Activations of the epilogues.  The first three codes are exposed by dwbc_debug_gemm / dwbc_debug_describe_chain; the hidden-layer
+// activations of rsl_rl's get_activation follow (DwbcNetCfg.activation maps onto them in mlp.cu).
+enum { ACT_NONE = 0, ACT_ELU = 1, ACT_TANH = 2, ACT_SELU = 3, ACT_RELU = 4, ACT_LRELU = 5, ACT_SIGMOID = 6 };
+constexpr float SELU_ALPHA = 1.6732632423543772f, SELU_SCALE = 1.0507009873554805f, LRELU_SLOPE = 0.01f;
+
+// tanh for the TF32 paths: 1 - 2/(e^{2x}+1) with ex2.approx / rcp.approx (a few ulp; saturates correctly at +-inf). Short enough that an
+// if-converted activation select costs nothing for the ELU layers (precise tanhf is ~60 predicated instructions per element).
+__device__ __forceinline__ float t2_tanh(float x) { return 1.0f - __fdividef(2.0f, __expf(2.0f * x) + 1.0f); }
+
+// f(x) of every activation: kFast = ex2.approx-based exp / tanh (TF32 paths, far below their input rounding); else precise expf / tanhf
+// (the fp32 anchor and the exact history encoder)
+template <bool kFast>
+__device__ __forceinline__ float act_f(int act, float x) {
+  switch (act) {
+    case ACT_ELU: return x > 0.0f ? x : (kFast ? __expf(x) : expf(x)) - 1.0f;
+    case ACT_SELU: return SELU_SCALE * (x > 0.0f ? x : SELU_ALPHA * ((kFast ? __expf(x) : expf(x)) - 1.0f));
+    case ACT_RELU: return fmaxf(x, 0.0f);
+    case ACT_LRELU: return x > 0.0f ? x : LRELU_SLOPE * x;
+    case ACT_TANH: return kFast ? t2_tanh(x) : tanhf(x);
+    case ACT_SIGMOID: return kFast ? __fdividef(1.0f, 1.0f + __expf(-x)) : 1.0f / (1.0f + expf(-x));
+    default: return x;
+  }
+}
+// f'(x) as a function of the OUTPUT y = f(x) alone (so a backward pass needs no stored pre-activation); at x = 0 the branch torch takes
+__device__ __forceinline__ float act_df(int act, float y) {
+  switch (act) {
+    case ACT_ELU: return y > 0.0f ? 1.0f : y + 1.0f;
+    case ACT_SELU: return y > 0.0f ? SELU_SCALE : y + SELU_SCALE * SELU_ALPHA;
+    case ACT_RELU: return y > 0.0f ? 1.0f : 0.0f;
+    case ACT_LRELU: return y > 0.0f ? 1.0f : LRELU_SLOPE;
+    case ACT_TANH: return 1.0f - y * y;
+    case ACT_SIGMOID: return y * (1.0f - y);
+    default: return 1.0f;
+  }
+}
 
 struct RowMat {
   const float* p;       // base (already offset to the first column)
@@ -39,8 +73,6 @@ inline RowMat rowmat_gather(const float* p, const int64_t* idx, int64_t stride) 
 inline RowMat rowmat_grouped(const float* p, const int64_t* idx, int rpg, int64_t stride_g, int64_t ld) {
   return RowMat{p, idx, rpg, stride_g, ld};
 }
-
-__device__ __forceinline__ float elu_f(float x) { return x > 0.0f ? x : expf(x) - 1.0f; }
 
 constexpr int GT_M = 64, GT_N = 64, GT_K = 16, GT_PAD = 4, GT_THREADS = 256;
 
@@ -188,12 +220,9 @@ __global__ void __launch_bounds__(GT_THREADS) gemm_tile_kernel(const GemmArgs g)
       if (g.beta) v += crow[n];
       if (kMode == GEMM_FWD) {
         if (g.bias) v += g.bias[n];
-        if (g.act == ACT_ELU) v = elu_f(v);
-        else if (g.act == ACT_TANH) v = tanhf(v);
+        v = act_f<false>(g.act, v);
       } else if (xrow) {
-        const float y = xrow[n];
-        if (g.act == ACT_ELU) v *= (y > 0.0f ? 1.0f : y + 1.0f);
-        else if (g.act == ACT_TANH) v *= (1.0f - y * y);
+        v *= act_df(g.act, xrow[n]);
       }
       crow[n] = v;
     }

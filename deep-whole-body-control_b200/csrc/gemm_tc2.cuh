@@ -3,7 +3,7 @@
 //
 //   warps 0-3  PRODUCERS : gather + pad the A operand of tile i+1 into shared-memory stage (i+1)%2 while ...
 //   warps 4-7  CONSUMERS : ... one warpgroup issues the wgmma chain of tile i (two 64-row halves), writes its accumulator
-//                          fragments over the consumed A stage and fuses bias / ELU / tanh / act' into coalesced row stores.
+//                          fragments over the consumed A stage and fuses bias / activation / act' into coalesced row stores.
 //
 //   FWD / BWD_DATA: CTA = persistent over 128-row tiles; weights (<= 64 KB) resident in smem; 2 A stages of 66 KB.
 //   BWD_WGT      : the grouped weight-gradient kernel (wgrad_group.cuh) with a single GEMM.
@@ -23,9 +23,6 @@ constexpr int T2_LDS = TC_MAXN + 4;                 // padded row stride (floats
 __device__ __forceinline__ void t2_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tc_smem_u32(bar)) : "memory");
 }
-// tanh for the TF32 path: 1 - 2/(e^{2x}+1) with ex2.approx / rcp.approx (a few ulp; saturates correctly at +-inf). Short enough that an
-// if-converted activation select costs nothing for the ELU layers (precise tanhf is ~60 predicated instructions per element).
-__device__ __forceinline__ float t2_tanh(float x) { return 1.0f - __fdividef(2.0f, __expf(2.0f * x) + 1.0f); }
 // named barriers are the warp-aligned form: reconverge the warp first (a lane may still be behind a single-lane mbarrier arrive)
 __device__ __forceinline__ void t2_pbar() { __syncwarp(); asm volatile("bar.sync 2, %0;" ::"n"(T2_PROD) : "memory"); }   // producers only
 __device__ __forceinline__ void t2_ebar() { __syncwarp(); asm volatile("bar.sync 3, %0;" ::"n"(T2_EPI) : "memory"); }    // epilogue only
@@ -267,10 +264,8 @@ __global__ void __launch_bounds__(T2_THREADS, 1) gemm_tc2_kernel(const GemmArgs 
               if (kMode == GEMM_FWD) {
                 tt += bias4[qq];
                 if (vecB & 8) { }
-                else if (g.act == ACT_ELU) tt = tt > 0.0f ? tt : __expf(tt) - 1.0f;   // ex2.approx: 2 ulp, far below the TF32 input rounding
-                else if (g.act == ACT_TANH) tt = t2_tanh(tt);
-              } else if (g.act == ACT_ELU) tt *= (y[u][qq] > 0.0f ? 1.0f : y[u][qq] + 1.0f);
-              else if (g.act == ACT_TANH) tt *= (1.0f - y[u][qq] * y[u][qq]);
+                else tt = act_f<true>(g.act, tt);   // ex2.approx: 2 ulp, far below the TF32 input rounding
+              } else if (g.act != ACT_NONE) tt *= act_df(g.act, y[u][qq]);
               x[u][qq] = tt;
             }
           }

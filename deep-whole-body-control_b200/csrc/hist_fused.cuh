@@ -26,10 +26,11 @@ struct HistFusedArgs {
   RowMat hist;                          // row r -> first float of its [10][76] history block
   float* out; int64_t ld_out;           // [rows, ld_out]; columns [latent, ld_out) are zero-filled
   int rows, latent;
+  int act;                              // hidden activation (ACT_*) after every layer (AC:49-73 apply the one activation throughout)
 };
 
-__device__ __forceinline__ float hf_elu(float x) { return x > 0.0f ? x : expf(x) - 1.0f; }     // precise expf: this is the exact path
-
+// kAct: the hidden activation, in its precise form (expf / tanhf): this is the exact path
+template <int kAct>
 __global__ void __launch_bounds__(HF_THREADS) hist_fused_kernel(const HistFusedArgs a) {
   __shared__ __align__(16) float w[HF_FLOATS];
   // ---- weights -> shared memory, transposed to [input][output] (pads zero) ----
@@ -81,7 +82,7 @@ __global__ void __launch_bounds__(HF_THREADS) hist_fused_kernel(const HistFusedA
       }
     }
 #pragma unroll
-    for (int o = 0; o < 30; ++o) h[o] = hf_elu(h[o]);
+    for (int o = 0; o < 30; ++o) h[o] = act_f<false>(kAct, h[o]);
     // ---- conv 1: step t is tap (t & 1) + 2 of position p - 1 and tap t & 1 of position p = t / 2 ----
     const int kb = t & 1, ka = kb + 2;
     if (t >= 2) {
@@ -115,7 +116,7 @@ __global__ void __launch_bounds__(HF_THREADS) hist_fused_kernel(const HistFusedA
         // position q = (t - 3) / 2 of conv 1 is complete
         const int q = (t - 3) >> 1;
 #pragma unroll
-        for (int o = 0; o < 20; ++o) c1a[o] = hf_elu(c1a[o]);
+        for (int o = 0; o < 20; ++o) c1a[o] = act_f<false>(kAct, c1a[o]);
         if (q >= 1) {
           // conv 2 position q - 1 = taps (c1[q-1], c1[q]); then its share of the output layer
           float c2[12];
@@ -135,7 +136,7 @@ __global__ void __launch_bounds__(HF_THREADS) hist_fused_kernel(const HistFusedA
           const float* wl = w + HF_WL + (q - 1) * 10 * 32;
 #pragma unroll
           for (int c = 0; c < 10; ++c) {
-            const float cv = hf_elu(c2[c]);
+            const float cv = act_f<false>(kAct, c2[c]);
             const float4* wr = reinterpret_cast<const float4*>(wl + c * 32);
 #pragma unroll
             for (int o4 = 0; o4 < 8; ++o4) {
@@ -155,13 +156,22 @@ __global__ void __launch_bounds__(HF_THREADS) hist_fused_kernel(const HistFusedA
   float* orow = a.out + (int64_t)r * a.ld_out;
 #pragma unroll
   for (int o = 0; o < 32; ++o)
-    if (o < a.ld_out) orow[o] = o < a.latent ? hf_elu(z[o]) : 0.0f;
+    if (o < a.ld_out) orow[o] = o < a.latent ? act_f<false>(kAct, z[o]) : 0.0f;
 }
 
 // latent <= 32, ld_out <= 32, history rows 16-byte aligned
 inline int launch_hist_fused(const HistFusedArgs& a, cudaStream_t st) {
   if (a.rows <= 0 || a.latent > 32 || a.ld_out > 32 || a.ld_out < a.latent) return DWBC_ERR_UNSUPPORTED;
-  hist_fused_kernel<<<(a.rows + HF_THREADS - 1) / HF_THREADS, HF_THREADS, 0, st>>>(a);
+  const unsigned grid = (a.rows + HF_THREADS - 1) / HF_THREADS;
+  switch (a.act) {
+    case ACT_ELU: hist_fused_kernel<ACT_ELU><<<grid, HF_THREADS, 0, st>>>(a); break;
+    case ACT_SELU: hist_fused_kernel<ACT_SELU><<<grid, HF_THREADS, 0, st>>>(a); break;
+    case ACT_RELU: hist_fused_kernel<ACT_RELU><<<grid, HF_THREADS, 0, st>>>(a); break;
+    case ACT_LRELU: hist_fused_kernel<ACT_LRELU><<<grid, HF_THREADS, 0, st>>>(a); break;
+    case ACT_TANH: hist_fused_kernel<ACT_TANH><<<grid, HF_THREADS, 0, st>>>(a); break;
+    case ACT_SIGMOID: hist_fused_kernel<ACT_SIGMOID><<<grid, HF_THREADS, 0, st>>>(a); break;
+    default: return DWBC_ERR_UNSUPPORTED;
+  }
   ++dwbc_launch_counter;
   return cudaGetLastError() == cudaSuccess ? DWBC_OK : DWBC_ERR_LAUNCH;
 }

@@ -215,15 +215,31 @@ __device__ __forceinline__ void c2_bias_act(float* v, const float* bias, int nva
         float e0, e1;
         c2_upk(c2_mul2(c2_pk(fminf(x0, 0.0f), fminf(x1, 0.0f)), l2e), e0, e1);
         c2_upk(c2_add2(c2_add2(c2_pk(c2_ex2(e0), c2_ex2(e1)), m1), c2_pk(fmaxf(x0, 0.0f), fmaxf(x1, 0.0f))), x0, x1);
+      } else if (kAct == ACT_SELU) {  // the same form scaled: s max(x,0) + s alpha (e^{min(x,0)} - 1)
+        const float e0 = c2_ex2(fminf(x0, 0.0f) * C2_LOG2E) - 1.0f, e1 = c2_ex2(fminf(x1, 0.0f) * C2_LOG2E) - 1.0f;
+        x0 = fmaf(SELU_SCALE * SELU_ALPHA, e0, SELU_SCALE * fmaxf(x0, 0.0f));
+        x1 = fmaf(SELU_SCALE * SELU_ALPHA, e1, SELU_SCALE * fmaxf(x1, 0.0f));
+      } else if (kAct != ACT_NONE) {
+        x0 = act_f<true>(kAct, x0); x1 = act_f<true>(kAct, x1);
       }
-      if (kAct == ACT_TANH) { x0 = t2_tanh(x0); x1 = t2_tanh(x1); }
       v[jj] = (kFull || jj < nvalid) ? x0 : 0.0f;
       v[jj + 1] = (kFull || jj + 1 < nvalid) ? x1 : 0.0f;
     }
   }
 }
+// v[jj] *= f'(y[jj]) over one 32-column chunk
+template <int kAct>
+__device__ __forceinline__ void c2_dact(float* v, const float* y) {
+#pragma unroll
+  for (int jj = 0; jj < 32; ++jj) v[jj] *= act_df(kAct, y[jj]);
+}
 __device__ __forceinline__ void c2_bias_act_any(float* v, const float* bias, int act, int nvalid) {
-  if (nvalid >= 32) {
+  if (act > ACT_TANH) {             // the other hidden activations: one masked form each (nvalid >= 32 masks nothing), to bound the code size
+    if (act == ACT_SELU) c2_bias_act<ACT_SELU, false>(v, bias, nvalid);
+    else if (act == ACT_RELU) c2_bias_act<ACT_RELU, false>(v, bias, nvalid);
+    else if (act == ACT_LRELU) c2_bias_act<ACT_LRELU, false>(v, bias, nvalid);
+    else c2_bias_act<ACT_SIGMOID, false>(v, bias, nvalid);
+  } else if (nvalid >= 32) {
     if (act == ACT_ELU) c2_bias_act<ACT_ELU, true>(v, bias, 32);
     else if (act == ACT_TANH) c2_bias_act<ACT_TANH, true>(v, bias, 32);
     else c2_bias_act<ACT_NONE, true>(v, bias, 32);
@@ -712,13 +728,20 @@ __global__ void __launch_bounds__(C2_THREADS, 1) chain2_kernel(const __grid_cons
                     }
                   }
                 }
-                if (use_x) {                                   // AC ELU / tanh derivatives from the layer's OUTPUTS
+                if (use_x) {                                   // activation derivatives from the layer's OUTPUTS (act_df)
                   if (o.act == ACT_TANH) {
-#pragma unroll
-                    for (int jj = 0; jj < 32; ++jj) v[jj] *= 1.0f - x[u][jj] * x[u][jj];
-                  } else {                                     // ELU'(y) = y > 0 ? 1 : y + 1 = min(y + 1, 1)
+                    c2_dact<ACT_TANH>(v, x[u]);
+                  } else if (o.act == ACT_ELU) {               // ELU'(y) = y > 0 ? 1 : y + 1 = min(y + 1, 1)
 #pragma unroll
                     for (int jj = 0; jj < 32; ++jj) v[jj] *= fminf(x[u][jj] + 1.0f, 1.0f);
+                  } else if (o.act == ACT_SELU) {
+                    c2_dact<ACT_SELU>(v, x[u]);
+                  } else if (o.act == ACT_RELU) {
+                    c2_dact<ACT_RELU>(v, x[u]);
+                  } else if (o.act == ACT_LRELU) {
+                    c2_dact<ACT_LRELU>(v, x[u]);
+                  } else {
+                    c2_dact<ACT_SIGMOID>(v, x[u]);
                   }
                 }
                 if (o.N - c0 < 32) {                           // ragged last chunk: the pad columns are operand columns of the next op

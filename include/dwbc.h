@@ -33,7 +33,7 @@ enum {
   DWBC_ERR_LAUNCH = -3       /* cudaGetLastError() != cudaSuccess after the launch */
 };
 
-#define DWBC_ABI_VERSION 3
+#define DWBC_ABI_VERSION 4
 #define DWBC_MAX_DOF 24
 #define DWBC_MAX_TERMS 40   /* active reward terms per channel */
 #define DWBC_MAX_IDX 8      /* penalised / termination contact bodies */
@@ -234,6 +234,18 @@ int dwbc_normalize_advantages(float* advantages, const double* stats, int64_t co
 
 #define DWBC_MAX_LAYERS 4
 
+/* Hidden-layer activation of the network (DwbcNetCfg.activation): the names of rsl_rl's get_activation.  The derivative of each is
+ * a function of the layer's output y alone, which is what every backward pass stores:
+ *   ELU      x > 0 ? x : e^x - 1                               y > 0 ? 1 : y + 1
+ *   SELU     s (x > 0 ? x : a (e^x - 1)), a = 1.6732632423543772, s = 1.0507009873554805
+ *                                                              y > 0 ? s : y + s a
+ *   RELU     max(x, 0)                                         y > 0 ? 1 : 0
+ *   LRELU    x > 0 ? x : 0.01 x  (nn.LeakyReLU())              y > 0 ? 1 : 0.01
+ *   TANH     tanh x                                            1 - y^2
+ *   SIGMOID  1 / (1 + e^-x)                                    y (1 - y)
+ * At x = 0 the derivative is the one torch uses (the negative branch, 0 for RELU). */
+enum DwbcActivation { DWBC_ACT_ELU = 0, DWBC_ACT_SELU, DWBC_ACT_RELU, DWBC_ACT_LRELU, DWBC_ACT_TANH, DWBC_ACT_SIGMOID };
+
 /* Network shape (AC:86-298).  Parameters live in ONE flat fp32 buffer in
  * ActorCritic.parameters() order (std first); offsets are element offsets into it. */
 typedef struct DwbcNetCfg {
@@ -261,7 +273,10 @@ typedef struct DwbcNetCfg {
    *   2  "3xTF32": every operand is split into the TF32 part the tensor core reads and the exact remainder, three tensor-core
    *      products per GEMM (hi*hi + lo*hi + hi*lo), fp32 accumulation: fp32-grade results on the tensor cores. */
   int32_t precision;
-  int32_t reserved_;
+  /* DwbcActivation after every hidden layer: privileged and history encoders (all four layers), both backbones and the hidden
+   * layers of the four heads.  The actor heads' outputs keep tanh, the critic heads' stay linear.  Other values:
+   * DWBC_ERR_UNSUPPORTED. */
+  int32_t activation;
 } DwbcNetCfg;
 
 /* PD torque controller of step() (WG:1262-1295 `_compute_torques`, called `decimation` times per policy step, WG:1175-1183):

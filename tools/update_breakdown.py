@@ -10,6 +10,7 @@ printed.  Needs a GPU: there is no fallback.
 
   python tools/update_breakdown.py --out bench_out/breakdown                                  # the built library
   python tools/update_breakdown.py --out bench_out/ab --lib old/libdwbc.so --lib new/libdwbc.so --rounds 2
+  python tools/update_breakdown.py --out bench_out/relu --activation relu                     # another hidden-layer activation
 """
 import argparse, json, os, re, statistics, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -38,9 +39,10 @@ def child(a):
     from torch.profiler import ProfilerActivity, profile
     if not torch.cuda.is_available():
         raise SystemExit("update_breakdown needs a CUDA device")
-    res = {"lib": _lib.LIB_PATH, "card": card(), "torch": torch.__version__, "precisions": {}}
+    res = {"lib": _lib.LIB_PATH, "activation": a.activation, "card": card(), "torch": torch.__version__, "precisions": {}}
     for prec in a.precisions:
-        ac = FlatActorCritic(device="cuda:0", seed=0, init_std=[[0.8, 1.0, 1.0] * 4 + [1.0] * 6], num_priv=24, num_hist=10, num_prop=76)
+        ac = FlatActorCritic(device="cuda:0", seed=0, init_std=[[0.8, 1.0, 1.0] * 4 + [1.0] * 6], num_priv=24, num_hist=10, num_prop=76,
+                             activation=a.activation)
         alg = FusedPPO(ac, device="cuda:0", precision=prec, num_learning_epochs=5, num_mini_batches=4, clip_param=0.2, gamma=0.99, lam=0.95,
                        learning_rate=2e-4, mixing_schedule=[1.0, 0, 1], priv_reg_coef_schedual=[0, 1, 1000, 1000])
         alg.init_storage(N_ENVS, T_STEPS, [860], [None], [18]); alg.counter = 1500
@@ -89,6 +91,7 @@ def main():
     ap.add_argument("--lib", action="append", default=[], help="libdwbc.so to measure; repeat to compare (default: the built one)")
     ap.add_argument("--rounds", type=int, default=1, help="times each library is measured (alternating)")
     ap.add_argument("--precisions", nargs="+", default=["tf32x3", "tf32"], choices=["tf32x3", "tf32"])
+    ap.add_argument("--activation", default="elu", help="hidden-layer activation of the network (rsl_rl name)")
     ap.add_argument("--top", type=int, default=8, help="kernels listed per table")
     ap.add_argument("--child", default=None, help=argparse.SUPPRESS)
     a = ap.parse_args()
@@ -100,11 +103,11 @@ def main():
     for rnd in range(a.rounds):
         for li, lib in enumerate(libs):
             path = os.path.join(a.out, f"run_r{rnd}_lib{li}.json")
-            cmd = [sys.executable, os.path.abspath(__file__), "--out", a.out, "--child", path, "--precisions", *a.precisions] + (["--lib", lib] if lib else [])
+            cmd = [sys.executable, os.path.abspath(__file__), "--out", a.out, "--child", path, "--precisions", *a.precisions, "--activation", a.activation] + (["--lib", lib] if lib else [])
             subprocess.run(cmd, check=True)                # no GPU / a failing library: the whole command fails
             runs.append((li, json.load(open(path))))
-    print("card (name, power limit, max SM clock):", runs[0][1]["card"])
-    summary = {"card": runs[0][1]["card"], "libs": [l or "built" for l in libs], "update_ms": {}}
+    print("card (name, power limit, max SM clock):", runs[0][1]["card"], "| activation:", a.activation)
+    summary = {"card": runs[0][1]["card"], "activation": a.activation, "libs": [l or "built" for l in libs], "update_ms": {}}
     for prec in a.precisions:
         for li, lib in enumerate(libs):
             sets = [x for i, r in runs if i == li for x in r["precisions"][prec]["update_ms_sets"]]
