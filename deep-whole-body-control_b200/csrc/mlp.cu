@@ -13,6 +13,7 @@
 #include "hist_fused.cuh"
 #include "mlp_chain2.cuh"
 #include "wgrad_group.cuh"
+#include "dwbc_debug.h"
 
 namespace dwbc {
 
@@ -1124,6 +1125,21 @@ extern "C" int dwbc_debug_set_chain_bwd_reverse(int on) {
 extern "C" int dwbc_debug_set_wgrad_reverse(int on) {
   wg_reverse = on ? 1 : 0;
   return DWBC_OK;
+}
+// The grouped weight-gradient launch on caller-described GEMMs (tests/test_gpu_wgrad_group.py)
+extern "C" int dwbc_debug_wgrad_group(const DwbcWgradGemm* gemms, int n, int rows, int x3, dwbc_stream_t stream) {
+  if (!gemms || n <= 0 || n > WG_MAX || rows <= 0) return DWBC_ERR_ARG;
+  auto mat = [](const float* p, const int64_t* idx, int image, int64_t ld) {
+    return image ? rowmat_image(p) : (idx ? rowmat_gather(p, idx, ld) : rowmat(p, ld));
+  };
+  WGroupBuilder b;
+  for (int i = 0; i < n; ++i) {
+    const DwbcWgradGemm& d = gemms[i];
+    if (!d.g || !d.x || !d.dw || (d.g_image && d.g_idx) || (d.x_image && d.x_idx)) return DWBC_ERR_ARG;
+    b.add(mat(d.g, d.g_idx, (int)d.g_image, d.g_ld), mat(d.x, d.x_idx, (int)d.x_image, d.x_ld), d.dw, d.lddw, d.db, (int)d.mo, (int)d.ni);
+  }
+  if (!b.ok) return DWBC_ERR_ARG;
+  return launch_wgrad_group(b.g, rows, x3 != 0, reinterpret_cast<cudaStream_t>(stream));
 }
 extern "C" int dwbc_debug_set_wgrad_items(int per_cta) {
   if (per_cta < 1 || per_cta > 64) return DWBC_ERR_ARG;

@@ -28,15 +28,25 @@ int dwbc_debug_describe_chain(const DwbcNetCfg* net, int32_t rows, int what, int
 /* the planner on its own (host code, no GPU): items per program and simulated makespans with / without one-tile items */
 int dwbc_debug_chain_plan(int tiles, int nprog, const double* cost, int sms, int* np2, int* ns1, double* span, double* span0);
 
-/* Deal of the grouped weight-gradient work items (wgrad_group.cuh): 0 = round-robin in construction order (default), 1 = GEMMs
- * sorted by operand width, items dealt boustrophedon (measured slower: all CTAs reduce into the same dW at the same time) */
+/* Deal of the grouped weight-gradient work items (wgrad_group.cuh), enumerated GEMM by GEMM, longest item first: 0 = round-robin
+ * (default), 1 = boustrophedon */
 int dwbc_debug_set_wgrad_snake(int on);
 /* tile order of the backward chain launch: 1 = from the last tile downwards (default), 0 = upwards */
 int dwbc_debug_set_chain_bwd_reverse(int on);
 /* slab order of the grouped weight-gradient launch: 1 = from the last rows downwards (default: the rows the backward chain touched last
  * are still in L2), 0 = upwards */
 int dwbc_debug_set_wgrad_reverse(int on);
-/* work items per CTA the slab length of the grouped weight-gradient launch aims at (default 4) */
+/* One GEMM of the grouped weight-gradient launch: dw[mo x ni] (row stride lddw) += G^T X and db[mo] += colsum(G) (db nullable) over
+ * `rows` rows of G [rows x mo] and X [rows x ni].  An operand is a tile image (*_image = 1: 128 columns, 64 KB per 128-row tile, idx
+ * NULL) or row-major with row stride *_ld, its rows optionally gathered through *_idx (row r is row idx[r] of the storage). */
+typedef struct {
+  const float* g; const int64_t* g_idx; int64_t g_image; int64_t g_ld;
+  const float* x; const int64_t* x_idx; int64_t x_image; int64_t x_ld;
+  float* dw; int64_t lddw; float* db; int64_t mo; int64_t ni;
+} DwbcWgradGemm;
+/* all n (<= 20) GEMMs in one launch, x3 = 1: 3xTF32, 0: TF32 */
+int dwbc_debug_wgrad_group(const DwbcWgradGemm* gemms, int n, int rows, int x3, dwbc_stream_t stream);
+/* work items per CTA of the grouped weight-gradient launch (default 4); more when items of equal cost would exceed 1024 rows */
 int dwbc_debug_set_wgrad_items(int per_cta);
 
 #ifdef __cplusplus
