@@ -635,12 +635,13 @@ extern "C" int dwbc_post_physics_step(const DwbcEnvCfg* cfg, const DwbcEnvBuffer
       !buf->obs_history || !buf->episode_sums || !buf->obs_buf || !buf->rew_buf || !buf->arm_rew_buf || !buf->reset_buf ||
       !buf->time_out_buf || !buf->episode_stats || (buf->store_rewards && !buf->store_values))
     return DWBC_ERR_ARG;
-  // v2 (32 envs per CTA, TMA bulk copies) whenever the shard is a multiple of 32 envs and every block is 16-B aligned
+  // both kernels move observation rows and history rows in 16-byte vectors
+  if (!aligned16(buf->obs_buf) || !aligned16(buf->obs_history)) return DWBC_ERR_UNSUPPORTED;
+  // v2 (16 envs per CTA, TMA bulk copies) whenever the shard is a multiple of 32 envs and every block is 16-B aligned
   if (cfg->num_envs % 32 == 0 && aligned16(buf->root_states) && aligned16(buf->dof_state) && aligned16(buf->force_sensor) &&
       aligned16(buf->torques) && aligned16(buf->actions) && aligned16(buf->action_history) && aligned16(buf->mass_params) &&
       aligned16(buf->friction) && aligned16(buf->motor_strength) && aligned16(buf->goal_state) && aligned16(buf->derived_state) &&
-      aligned16(buf->episode_length) && aligned16(buf->obs_history) && aligned16(buf->episode_sums) && aligned16(buf->obs_buf) &&
-      !args->generic_kernel) {
+      aligned16(buf->episode_length) && aligned16(buf->episode_sums) && !args->generic_kernel) {
     int rc = dwbc_launch_env_step_v2(cfg, buf, args, (cudaStream_t)stream);
     if (rc != DWBC_ERR_UNSUPPORTED) return rc;
   }

@@ -1,4 +1,4 @@
-// Fused widowGo1 post-physics step, v2: ONE launch per sim step, 32 envs per CTA, TMA-fed.
+// Fused widowGo1 post-physics step, v2: ONE launch per sim step, 16 envs per CTA, TMA-fed.
 //
 //  * Every contiguous block of the CTA's 32 envs (history rows 97 KB, root / dof / sensor / torque /
 //    action blocks, packed task-state rows, episode sums) is fetched with a 1-D TMA bulk copy

@@ -162,7 +162,9 @@ class FusedWidowGo1Core:
         self._cfg = make_env_cfg(p, self._sums_stride)
         self._buf = L.EnvBuffers()
         self._args = L.StepArgs()
-        self._args.generic_kernel = int(generic_kernel)     # True: always the warp-per-env kernel (the fallback for odd N / unaligned buffers)
+        # True: always the warp-per-env kernel, which also runs by itself when N is not a multiple of 32 or a state row block is not
+        # 16-byte aligned (the observation target and the history must be 16-byte aligned for both kernels)
+        self._args.generic_kernel = int(generic_kernel)
         self._leg_terms, self._arm_terms = p.active_terms("leg"), p.active_terms("arm")
         if state is not None:
             self.load_state(state)
@@ -207,7 +209,15 @@ class FusedWidowGo1Core:
     rigid_body_state = property(lambda s: s._rigid_body_state[:, :-1, :])
     contact_forces = property(lambda s: s._contact_forces[:, :-1, :])
     ee_pos = property(lambda s: s._rigid_body_state[:, s.p.gripper_idx, :3])
-    obs_history_buf = property(lambda s: s._hist)
+
+    @property
+    def obs_history_buf(self):
+        """[N, history_len, num_prop] proprioception history, stored unclipped as in the reference.  The TMA kernel keeps a per-env
+        count of the most recent history rows known to lie within +-clip_observations (derived_state column 27) and skips the
+        clipping of obs[:, 100:] while that count covers the whole history; `load_state` resets the count.  A write into this
+        tensor from outside (anything but `load_state`) must not store a value beyond +-clip_observations, or the next
+        observations may carry it unclipped."""
+        return self._hist
 
     @property
     def episode_length_buf(self):
@@ -257,7 +267,19 @@ class FusedWidowGo1Core:
 
     def set_obs_target(self, tensor: Optional[torch.Tensor]):
         """Direct the kernel's observation output to `tensor` ([N, >=num_obs] row-major), e.g. a row
-        of RolloutStorage.observations (SURVEY f2: saves the RS:98 copy)."""
+        of RolloutStorage.observations (SURVEY f2: saves the RS:98 copy).  The kernels write whole rows in 16-byte vectors, so the
+        target must be float32 on this core's device with unit column stride, a 16-byte-aligned start and a row stride that is a
+        multiple of 4 floats; anything else raises DwbcError here instead of reaching the kernel."""
+        if tensor is not None:
+            if tensor.dtype != torch.float32 or tensor.device.type != self.device.type or \
+                    (self.device.index is not None and tensor.device.index != self.device.index):
+                raise L.DwbcError(f"obs target must be float32 on {self.device}, got {tensor.dtype} on {tensor.device}")
+            if tensor.dim() != 2 or tensor.shape[0] != self.num_envs or tensor.shape[1] < self.num_obs or tensor.stride(1) != 1:
+                raise L.DwbcError(f"obs target must be [{self.num_envs}, >={self.num_obs}] with unit column stride, "
+                                  f"got shape {tuple(tensor.shape)} strides {tensor.stride()}")
+            if tensor.data_ptr() % 16 or tensor.stride(0) % 4:
+                raise L.DwbcError(f"obs target must start 16-byte aligned with a row stride that is a multiple of 4 floats, "
+                                  f"got address {tensor.data_ptr():#x} and row stride {tensor.stride(0)}")
         self.obs_buf = self._obs_own if tensor is None else tensor
         self._buf.obs_buf = self.obs_buf.data_ptr()
         self._buf.obs_stride = self.obs_buf.stride(0)

@@ -158,8 +158,8 @@ typedef struct DwbcEnvBuffers {
   const int64_t* terrain_types;  /* [N] */
   const float* terrain_origins;  /* [max_terrain_level,terrain_n_types,3] */
   /* outputs */
-  float* obs_buf;                /* [N,obs_stride] */
-  int64_t obs_stride;            /* row stride in floats (num_obs, or more when writing into storage) */
+  float* obs_buf;                /* [N,obs_stride], 16-byte aligned (obs_history too): else DWBC_ERR_UNSUPPORTED */
+  int64_t obs_stride;            /* row stride in floats (num_obs, or more when writing into storage), a multiple of 4 */
   float* rew_buf;                /* [N] */
   float* arm_rew_buf;            /* [N] */
   uint8_t* reset_buf;            /* [N] torch.bool */
@@ -185,7 +185,9 @@ typedef struct DwbcStepArgs {
   float lin_vel_x[2], ang_vel_yaw[2], goal_l[2], goal_p[2], goal_y[2]; /* (lo, span=hi-lo) */
   float leg_scale[DWBC_MAX_TERMS], arm_scale[DWBC_MAX_TERMS];         /* aligned with cfg.leg_term / arm_term */
   float leg_termination_scale, arm_termination_scale;                  /* 0 when inactive */
-  int32_t generic_kernel;        /* 1 = always run the warp-per-env kernel (any N / unaligned buffers), 0 = pick by shape */
+  int32_t generic_kernel;        /* 1 = always run the warp-per-env kernel (any N; only obs_buf and obs_history must be 16-B aligned),
+                                    0 = pick by shape: the 16-envs-per-CTA TMA kernel when N is a multiple of 32 and every row block
+                                    is 16-B aligned, else the warp-per-env kernel */
   int32_t reserved_;
 } DwbcStepArgs;
 

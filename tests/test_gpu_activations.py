@@ -267,7 +267,13 @@ def test_update_end_to_end_matches_oracle(activation, precision):
 
     res = alg.update(indices=perm.cuda(), on_step=on_step)
     # float64 oracle: with leaky ReLU, the float32 oracle on the CPU is itself 1.8e-4 away from float64 in 0.13 % of the parameters after
-    # 20 steps (rows on the other side of the kink), and the GPU agrees with float64 there
+    # 20 steps: a pre-activation of this data set lies within float32 rounding of the kink, and which side float32 arithmetic puts it on
+    # depends on the summation order.  The GPU's weight gradients are summed with split-K atomics (order varies from run to run), so
+    # its 20-step parameters follow one of the two trajectories: the float64 one or the float32 oracle's.  The float32 oracle is the same
+    # update in the GPU's precision, so the 20-step parameters must match one of the two references at the full tolerance.
+    P32 = {k: v.clone().float() for k, v in P.items()}
+    with oracle_activation(activation):
+        PO.ppo_update(P32, PO.Adam(list(P32.keys()), hp["learning_rate"]), {k: v.float() for k, v in st.items()}, perm, hp, COUNTER)
     Po = {k: v.double() for k, v in P.items()}
     st = {k: v.double() for k, v in st.items()}
     ref1 = {}
@@ -283,10 +289,15 @@ def test_update_end_to_end_matches_oracle(activation, precision):
     # Adam's step is ~lr * g / (|g| + 1e-8): an entry whose gradient is ~1e-8 (tanh / leaky-ReLU units deep in saturation) moves by up to
     # lr whatever the arithmetic (test_gpu_ppo.py: "bounded by 2*lr").  Every other entry agrees to 2e-5; such entries are rare.
     d1 = torch.cat([(snap["p1"][n].cpu() - ref1[n]).abs().reshape(-1) for n in ref1])
-    d20 = torch.cat([(ac.unflat(ac.flat)[n].cpu() - Po[n]).abs().reshape(-1) for n in Po])
-    f1, f20 = float((d1 > 2e-5).float().mean()), float((d20 > 2e-5).float().mean())
+    got = ac.unflat(ac.flat)
+    d20_64 = torch.cat([(got[n].cpu() - Po[n]).abs().reshape(-1) for n in Po])
+    d20_32 = torch.cat([(got[n].cpu() - P32[n]).abs().reshape(-1) for n in Po])
+    f1 = float((d1 > 2e-5).float().mean())
+    f20_64, f20_32 = float((d20_64 > 2e-5).float().mean()), float((d20_32 > 2e-5).float().mean())
+    d20, f20 = (d20_64, f20_64) if f20_64 <= f20_32 else (d20_32, f20_32)
     print(f"[{activation} {precision}] update(): losses {res[0] - o_val:+.3g} {res[1] - o_sur:+.3g}; params max abs error after 1 step "
-          f"{float(d1.max()):.3g} (fraction beyond 2e-5: {f1:.2g}), after 20 steps {float(d20.max()):.3g} ({f20:.2g})")
+          f"{float(d1.max()):.3g} (fraction beyond 2e-5: {f1:.2g}), after 20 steps {float(d20.max()):.3g} ({f20:.2g}); "
+          f"fraction beyond 2e-5 after 20 steps vs float64 {f20_64:.2g}, vs the float32 oracle {f20_32:.2g}")
     assert abs(res[0] - o_val) < 2e-5 * max(1.0, abs(o_val)) and abs(res[1] - o_sur) < 2e-5
     assert float(d1.max()) < 2 * hp["learning_rate"] and float(d20.max()) < 2 * hp["learning_rate"]
     assert f1 < 1e-4 and f20 < 1e-4
