@@ -12,7 +12,7 @@ import subprocess
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libdwbc.so")
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 MAX_DOF, MAX_TERMS, MAX_IDX, MAX_SLOTS, NUM_METRICS, RAND_COLS, MAX_LAYERS = 24, 40, 8, 64, 10, 104, 4
 GS, DS = 28, 72
 GS_COL = dict(commands=0, goal_timer=3, traj_timesteps=4, traj_total_timesteps=5, ee_start_sphere=6, ee_goal_sphere=9,
@@ -84,9 +84,10 @@ class NetCfg(C.Structure):
         ("n_leg_layers", i32), ("leg_dims", i32 * MAX_LAYERS),
         ("n_arm_layers", i32), ("arm_dims", i32 * MAX_LAYERS),
         ("hist_proj", i32), ("hist_c1", i32), ("hist_k1", i32), ("hist_s1", i32), ("hist_c2", i32), ("hist_k2", i32), ("hist_s2", i32),
+        ("hist_c3", i32), ("hist_k3", i32), ("hist_s3", i32), ("n_hist_conv", i32),
         ("num_params", i64), ("off_std", i64),
         ("off_priv_w", i64 * MAX_LAYERS), ("off_priv_b", i64 * MAX_LAYERS),
-        ("off_hist_w", i64 * 4), ("off_hist_b", i64 * 4),
+        ("off_hist_w", i64 * 5), ("off_hist_b", i64 * 5),
         ("off_actor_w", i64 * MAX_LAYERS), ("off_actor_b", i64 * MAX_LAYERS),
         ("off_aleg_w", i64 * (MAX_LAYERS + 1)), ("off_aleg_b", i64 * (MAX_LAYERS + 1)),
         ("off_aarm_w", i64 * (MAX_LAYERS + 1)), ("off_aarm_b", i64 * (MAX_LAYERS + 1)),

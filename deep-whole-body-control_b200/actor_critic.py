@@ -19,6 +19,17 @@ from . import _lib as L
 
 ALIGN = 32
 
+# StateHistoryEncoder conv stacks by tsteps = num_hist (AC:52-70): (out_channels, kernel, stride) of conv_layers.0, .2 (, .4).  Every
+# stack ends at 3 positions x 10 channels, the 30 inputs of linear_output; any other num_hist raises, as the reference does.
+HIST_CONVS = {10: ((20, 4, 2), (10, 2, 1)), 20: ((20, 6, 2), (10, 4, 2)), 50: ((20, 8, 4), (10, 5, 1), (10, 5, 1))}
+HIST_PROJ = 30
+
+
+def hist_convs(num_hist):
+    if num_hist not in HIST_CONVS:
+        raise L.DwbcError(f"num_hist={num_hist}: the history encoder exists for tsteps in {sorted(HIST_CONVS)} (AC:52-70)")
+    return HIST_CONVS[num_hist]
+
 
 def manifest(num_prop=76, num_priv=24, num_hist=10, priv_dims=(64, 20), actor_dims=(128,), critic_dims=(128,),
              leg_dims=(128, 128), arm_dims=(128, 128), n_leg=12, n_arm=6) -> List[Tuple[str, tuple]]:
@@ -33,10 +44,12 @@ def manifest(num_prop=76, num_priv=24, num_hist=10, priv_dims=(64, 20), actor_di
         lin("actor.priv_encoder", 2 * k, o, d)
         d = o
     latent = d
-    lin("actor.history_encoder.encoder", 0, 30, num_prop)                               # AC:49-51
-    m += [("actor.history_encoder.conv_layers.0.weight", (20, 30, 4)), ("actor.history_encoder.conv_layers.0.bias", (20,)),
-          ("actor.history_encoder.conv_layers.2.weight", (10, 20, 2)), ("actor.history_encoder.conv_layers.2.bias", (10,))]  # AC:58-62
-    lin("actor.history_encoder.linear_output", 0, latent, 30)                           # AC:71-73
+    lin("actor.history_encoder.encoder", 0, HIST_PROJ, num_prop)                        # AC:49-51
+    cin = HIST_PROJ
+    for k, (co, ks, _) in enumerate(hist_convs(num_hist)):                              # AC:52-70
+        m += [(f"actor.history_encoder.conv_layers.{2 * k}.weight", (co, cin, ks)), (f"actor.history_encoder.conv_layers.{2 * k}.bias", (co,))]
+        cin = co
+    lin("actor.history_encoder.linear_output", 0, latent, 3 * cin)                      # AC:71-73
     d = num_prop + latent
     for k, o in enumerate(actor_dims):
         lin("actor.actor_backbone", 2 * k, o, d)
@@ -122,7 +135,10 @@ class FlatActorCritic:
         dims("n_critic_layers", "critic_dims", self.critic_dims)
         dims("n_leg_layers", "leg_dims", self.leg_dims)
         dims("n_arm_layers", "arm_dims", self.arm_dims)
-        c.hist_proj, c.hist_c1, c.hist_k1, c.hist_s1, c.hist_c2, c.hist_k2, c.hist_s2 = 30, 20, 4, 2, 10, 2, 1
+        convs = hist_convs(self.num_hist)
+        c.hist_proj, c.n_hist_conv = HIST_PROJ, len(convs)
+        for k, (co, ks, st) in enumerate(convs):
+            setattr(c, f"hist_c{k + 1}", co); setattr(c, f"hist_k{k + 1}", ks); setattr(c, f"hist_s{k + 1}", st)  # noqa: E702
         c.num_params, c.off_std = self.num_params, o["std"]
         c.activation = L.ACTIVATIONS[self.activation]
 
@@ -131,9 +147,10 @@ class FlatActorCritic:
                 getattr(c, w_attr)[i] = o[f"{prefix}.{2 * i}.weight"]
                 getattr(c, b_attr)[i] = o[f"{prefix}.{2 * i}.bias"]
         offs("off_priv_w", "off_priv_b", "actor.priv_encoder", len(self.priv_dims))
-        for i, k in enumerate(("encoder.0", "conv_layers.0", "conv_layers.2", "linear_output.0")):
-            c.off_hist_w[i] = o[f"actor.history_encoder.{k}.weight"]
-            c.off_hist_b[i] = o[f"actor.history_encoder.{k}.bias"]
+        for i, k in enumerate(("encoder.0", "conv_layers.0", "conv_layers.2", "conv_layers.4", "linear_output.0")):
+            present = f"actor.history_encoder.{k}.weight" in o                              # conv_layers.4: 50-step stack only
+            c.off_hist_w[i] = o[f"actor.history_encoder.{k}.weight"] if present else -1
+            c.off_hist_b[i] = o[f"actor.history_encoder.{k}.bias"] if present else -1
         offs("off_actor_w", "off_actor_b", "actor.actor_backbone", len(self.actor_dims))
         offs("off_aleg_w", "off_aleg_b", "actor.actor_leg_control_head", len(self.leg_dims) + 1)
         offs("off_aarm_w", "off_aarm_b", "actor.actor_arm_control_head", len(self.arm_dims) + 1)

@@ -22,7 +22,7 @@
 namespace dwbc {
 
 constexpr int ENV_WARPS = 4;
-constexpr int MAX_H4 = 8;  // history row <= 8*32 float4 = 1024 floats
+constexpr int MAX_H4 = 8;  // history row <= 8*32 float4 = 1024 floats in registers; longer rows take the streaming form (kLong)
 
 // shared-memory staging block of one warp (float offsets)
 enum {
@@ -260,6 +260,11 @@ __device__ float eval_term(int term, const TermCtx& c) {
   return r;
 }
 
+// kLong = false: the history row (<= 1024 floats) is loaded into registers before anything else and re-emitted from there.
+// kLong = true (history_len * num_prop > 1024, e.g. 20 or 50 steps of 76): the row is streamed at the end instead, in ascending
+// 32-float4 chunks: each chunk is loaded, written to obs clipped (WG:992, 1195-1196), and after a __syncwarp written back one num_prop
+// row lower (WG:997-999).  In place is safe: the targets of chunk i lie below its end, so chunks <= i have read them already.
+template <bool kLong>
 __global__ void __launch_bounds__(ENV_WARPS * 32)
 env_step_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant__ DwbcEnvBuffers B,
                 const __grid_constant__ DwbcStepArgs A) {
@@ -275,11 +280,14 @@ env_step_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant__ 
 
   // ---- 1. history row: all 128-bit loads in flight first --------------------------------------
   float4* hist4 = reinterpret_cast<float4*>(B.obs_history + (size_t)e * H * P);
-  float4 h[MAX_H4];
+  float4 h[kLong ? 1 : MAX_H4];
+  bool hist_zeroed = false;                  // (kLong) reset this step: the old history reads as zeros (WG:735)
+  if constexpr (!kLong) {
 #pragma unroll
-  for (int i = 0; i < MAX_H4; ++i) {
-    int idx = lane + 32 * i;
-    h[i] = idx < nh4 ? ldg_stream(hist4 + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int i = 0; i < MAX_H4; ++i) {
+      int idx = lane + 32 * i;
+      h[i] = idx < nh4 ? ldg_stream(hist4 + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
   }
   // ---- 2. coalesced staging of the env's small inputs ------------------------------------------
   float* root_g = B.root_states + (size_t)e * 26;
@@ -479,8 +487,12 @@ env_step_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant__ 
     if (lane < 4) sm[S_DS + DWBC_DS_FEET_AIR_TIME + lane] = 0.0f;
     if (lane < na) sm[S_AH + lane] = 0.0f;
     for (int i = lane; i < cfg.action_hist_len * na; i += 32) ah_g[i] = 0.0f;
+    if constexpr (!kLong) {
 #pragma unroll
-    for (int i = 0; i < MAX_H4; ++i) h[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int i = 0; i < MAX_H4; ++i) h[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    } else {
+      hist_zeroed = true;
+    }
     ep = 0;
     // extras['episode'] means (WG:743-750): sum over reset envs via atomics, divided on the host
     for (int i = lane; i < nslots; i += 32) {
@@ -535,25 +547,41 @@ env_step_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant__ 
   const float4* prop4 = reinterpret_cast<const float4*>(sm + S_PROP);
   const float4* priv4 = reinterpret_cast<const float4*>(sm + S_PRIV);
   if (lane < pp4) stg_stream(obs4 + lane, clip4(lane < p4 ? prop4[lane] : priv4[lane - p4], c));
-#pragma unroll
-  for (int i = 0; i < MAX_H4; ++i) {
-    int idx = lane + 32 * i;
-    if (idx < nh4) stg_stream(obs4 + pp4 + idx, clip4(h[i], c));  // OLD history (WG:992)
-  }
-  __syncwarp();  // every lane's history loads have been consumed: the in-place shift below is safe
-  if (ep <= 1) {  // WG:994-996: fill all H rows with the new proprioception
+  if constexpr (!kLong) {
 #pragma unroll
     for (int i = 0; i < MAX_H4; ++i) {
       int idx = lane + 32 * i;
-      if (idx < nh4) hist4[idx] = prop4[idx % p4];
+      if (idx < nh4) stg_stream(obs4 + pp4 + idx, clip4(h[i], c));  // OLD history (WG:992)
     }
-  } else {        // WG:997-1000: drop the oldest row, append
+    __syncwarp();  // every lane's history loads have been consumed: the in-place shift below is safe
+    if (ep <= 1) {  // WG:994-996: fill all H rows with the new proprioception
 #pragma unroll
-    for (int i = 0; i < MAX_H4; ++i) {
-      int idx = lane + 32 * i;
-      if (idx >= p4 && idx < nh4) hist4[idx - p4] = h[i];
+      for (int i = 0; i < MAX_H4; ++i) {
+        int idx = lane + 32 * i;
+        if (idx < nh4) hist4[idx] = prop4[idx % p4];
+      }
+    } else {        // WG:997-1000: drop the oldest row, append
+#pragma unroll
+      for (int i = 0; i < MAX_H4; ++i) {
+        int idx = lane + 32 * i;
+        if (idx >= p4 && idx < nh4) hist4[idx - p4] = h[i];
+      }
+      if (lane < p4) hist4[nh4 - p4 + lane] = prop4[lane];
     }
-    if (lane < p4) hist4[nh4 - p4 + lane] = prop4[lane];
+  } else {
+    const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int i0 = 0; i0 < nh4; i0 += 32) {
+      const int idx = i0 + lane;
+      h[0] = idx < nh4 && !hist_zeroed ? __ldcs(hist4 + idx) : zero4;
+      if (idx < nh4) stg_stream(obs4 + pp4 + idx, clip4(h[0], c));    // OLD history (WG:992)
+      __syncwarp();  // the whole chunk has been read: its targets (and everything below them) may be overwritten
+      if (ep <= 1) {          // WG:994-996
+        if (idx < nh4) hist4[idx] = prop4[idx % p4];
+      } else if (idx >= p4 && idx < nh4) {
+        hist4[idx - p4] = h[0];                                            // WG:997-999
+      }
+    }
+    if (ep > 1 && lane < p4) hist4[nh4 - p4 + lane] = prop4[lane];          // WG:1000
   }
   if (lane < DWBC_GS) gs_g[lane] = sm[S_GS + lane];
   for (int i = lane; i < DWBC_DS; i += 32) ds_g[i] = sm[S_DS + i];
@@ -621,7 +649,7 @@ extern "C" int dwbc_post_physics_step(const DwbcEnvCfg* cfg, const DwbcEnvBuffer
   if (cfg->num_prop != 2 + 3 + 2 * nd + na + 4 + 3 + 3 + 3) return DWBC_ERR_UNSUPPORTED;  // WG:973-983
   if (cfg->num_priv != 5 + 1 + na) return DWBC_ERR_UNSUPPORTED;                            // WG:987-991
   if ((cfg->num_prop & 3) || (cfg->num_priv & 3) || (buf->obs_stride & 3)) return DWBC_ERR_UNSUPPORTED;
-  if (cfg->num_prop > 96 || cfg->history_len * cfg->num_prop > MAX_H4 * 128) return DWBC_ERR_UNSUPPORTED;
+  if (cfg->num_prop > 96 || cfg->history_len < 1) return DWBC_ERR_UNSUPPORTED;
   if (cfg->n_sum_slots + DWBC_NUM_METRICS > DWBC_MAX_SLOTS || cfg->sums_stride < cfg->n_sum_slots + DWBC_NUM_METRICS) return DWBC_ERR_ARG;
   if (cfg->n_leg_terms > DWBC_MAX_TERMS || cfg->n_arm_terms > DWBC_MAX_TERMS) return DWBC_ERR_ARG;
   if (cfg->n_penalized > DWBC_MAX_IDX || cfg->n_term_contact > DWBC_MAX_IDX) return DWBC_ERR_ARG;
@@ -646,7 +674,10 @@ extern "C" int dwbc_post_physics_step(const DwbcEnvCfg* cfg, const DwbcEnvBuffer
     if (rc != DWBC_ERR_UNSUPPORTED) return rc;
   }
   const int grid = (cfg->num_envs + ENV_WARPS - 1) / ENV_WARPS;
-  env_step_kernel<<<grid, ENV_WARPS * 32, 0, (cudaStream_t)stream>>>(*cfg, *buf, *args);
+  if ((int64_t)cfg->history_len * cfg->num_prop <= MAX_H4 * 128)
+    env_step_kernel<false><<<grid, ENV_WARPS * 32, 0, (cudaStream_t)stream>>>(*cfg, *buf, *args);
+  else
+    env_step_kernel<true><<<grid, ENV_WARPS * 32, 0, (cudaStream_t)stream>>>(*cfg, *buf, *args);
   DWBC_LAUNCH_CHECK();
   return DWBC_OK;
 }

@@ -51,12 +51,11 @@ struct Plan {
   float* cl[DWBC_MAX_LAYERS];
   float* ca[DWBC_MAX_LAYERS];
   float* value;                   // [rows, 2]
-  // history encoder
+  // history encoder (HistGeo: conv i reads rows of width ld[i] and writes positions pos[i + 1] x ld[i + 1])
   float* hproj;                   // [rows*T, 32]
-  float* hc1;                     // [rows*4, 20]
-  float* hc2;                     // [rows*3, 12]
+  float* hc[3];                   // conv outputs [rows*pos[i+1], ld[i+1]]: [rows*P1, 20], [rows*P2, 12] (, [rows*3, 12])
   float* zh;                      // [rows, latent]
-  float* hw1; float* hw2; float* hwl;      // re-packed weights
+  float* hw[3]; float* hwl;                // re-packed weights: conv i [c_i][k_i*ld[i]], linear_output [32][36]
   float* wpack;                            // packed weight images of the fused chain kernels (mlp_chain2.cuh)
   int* queue;                              // work-item counters of the chain kernel (zero between launches)
   // gradients
@@ -67,12 +66,49 @@ struct Plan {
   float* d0; float* d1; float* d2;         // ping-pong [rows, maxw]
   float* dz;                               // [rows, latent]
   float* dzh;                              // [rows, latent] (dagger)
-  float* dh_a1; float* dh_a2;              // im2col-space grads of the conv inputs (dagger)
-  float* dh_c1; float* dh_proj;
-  float* dhw1; float* dhw2; float* dhwl;   // grads of the re-packed weights (dagger)
+  float* dh_a[3];                          // im2col-space grads of the conv inputs (dagger) [rows*pos[i+1], k_i*ld[i]]
+  float* dh_c[2]; float* dh_proj;          // grads of the conv-2 / conv-3 inputs [rows*pos[i], ld[i]] and of the projection
+  float* dhw[3]; float* dhwl;              // grads of the re-packed weights (dagger)
   int mean_ld, maxw, latent;
   int64_t bytes;
 };
+
+// The history encoder's variant (a row of HIST_VARIANTS, hist_fused.cuh) with the row widths of the layer-wise path: the projection
+// is padded to 32 channels (so 10 steps keep K = 128 for conv 1), conv-1 outputs are 20 wide, later conv outputs 12 (linear_output
+// reads 3 x 12).  Conv i is one GEMM over overlapping windows: output position p of a row reads the k_i * ld[i] contiguous floats
+// from input position p * s_i on.
+struct HistGeo {
+  int var, T, nconv;
+  int c[3], k[3], s[3];
+  int cin[3], ld[4], pos[4];
+  int kdim(int i) const { return k[i] * ld[i]; }
+};
+static int hist_variant(const DwbcNetCfg& n) {
+  for (int v = 0; v < HIST_NVAR; ++v) {
+    const HistVariant& h = HIST_VARIANTS[v];
+    if (n.num_hist != h.T || n.n_hist_conv != h.nconv || n.hist_proj != HIST_PROJ) continue;
+    const int32_t got[9] = {n.hist_c1, n.hist_k1, n.hist_s1, n.hist_c2, n.hist_k2, n.hist_s2, n.hist_c3, n.hist_k3, n.hist_s3};
+    bool ok = true;
+    for (int i = 0; i < 3; ++i) ok = ok && got[3 * i] == h.c[i] && got[3 * i + 1] == h.k[i] && got[3 * i + 2] == h.s[i];
+    if (ok) return v;
+  }
+  return -1;
+}
+static HistGeo hist_geo(const DwbcNetCfg& n) {
+  HistGeo g{};
+  g.var = hist_variant(n);
+  if (g.var < 0) return g;                  // (every entry point has refused such a net in check_net)
+  const HistVariant& h = HIST_VARIANTS[g.var];
+  g.T = h.T; g.nconv = h.nconv;
+  g.pos[0] = h.T; g.ld[0] = 32;
+  for (int i = 0; i < h.nconv; ++i) {
+    g.c[i] = h.c[i]; g.k[i] = h.k[i]; g.s[i] = h.s[i];
+    g.cin[i] = i == 0 ? HIST_PROJ : h.c[i - 1];
+    g.ld[i + 1] = i == 0 ? 20 : 12;
+    g.pos[i + 1] = hist_out_len(g.pos[i], h.k[i], h.s[i]);
+  }
+  return g;
+}
 
 static int maxdim(const DwbcNetCfg& n) {
   int m = 32;
@@ -105,11 +141,14 @@ static Plan make_plan(const DwbcNetCfg& n, int64_t rows, void* ws) {
   for (int i = 0; i < n.n_leg_layers; ++i) p.cl[i] = b.f(act_floats(rows, n.leg_dims[i]));
   for (int i = 0; i < n.n_arm_layers; ++i) p.ca[i] = b.f(act_floats(rows, n.arm_dims[i]));
   p.value = b.f(rows * 2);
+  const HistGeo g = hist_geo(n);
+  const bool c3 = g.nconv == 3;            // (the absent third conv takes no space: the 10-step plan is the one it always was)
   p.hproj = b.f(rows * n.num_hist * 32);
-  p.hc1 = b.f(rows * 4 * 20);
-  p.hc2 = b.f(rows * 3 * 12);
+  for (int i = 0; i < 3; ++i) p.hc[i] = b.f(i < g.nconv ? rows * g.pos[i + 1] * g.ld[i + 1] : 0);
   p.zh = b.f(rows * align_up(p.latent, 4));
-  p.hw1 = b.f(20 * 128); p.hw2 = b.f(10 * 40); p.hwl = b.f(32 * 36);
+  for (int i = 0; i < 2; ++i) p.hw[i] = b.f(g.c[i] * g.kdim(i));
+  p.hw[2] = b.f(c3 ? g.c[2] * g.kdim(2) : 0);
+  p.hwl = b.f(32 * 36);
   p.wpack = b.f(C2_PACK_FLOATS);
   p.g_leg = b.f(rows * align_up(n.n_leg, 4)); p.g_arm = b.f(rows * align_up(n.n_arm, 4));
   p.g_vl = b.f(rows * 4); p.g_va = p.g_vl ? p.g_vl + 1 : nullptr; p.g_z = b.f(rows * align_up(p.latent, 4));
@@ -121,9 +160,12 @@ static Plan make_plan(const DwbcNetCfg& n, int64_t rows, void* ws) {
   p.d0 = b.f(rows * p.maxw); p.d1 = b.f(rows * p.maxw); p.d2 = b.f(rows * p.maxw);
   p.dz = b.f(rows * align_up(p.latent, 4));
   p.dzh = b.f(rows * align_up(p.latent, 4));
-  p.dh_a1 = b.f(rows * 4 * 128); p.dh_a2 = b.f(rows * 3 * 40);
-  p.dh_c1 = b.f(rows * 4 * 20); p.dh_proj = b.f(rows * n.num_hist * 32);
-  p.dhw1 = b.f(20 * 128); p.dhw2 = b.f(10 * 40); p.dhwl = b.f(32 * 36);
+  for (int i = 0; i < 3; ++i) p.dh_a[i] = b.f(i < g.nconv ? rows * g.pos[i + 1] * g.kdim(i) : 0);
+  p.dh_c[0] = b.f(rows * g.pos[1] * g.ld[1]);
+  p.dh_c[1] = b.f(c3 ? rows * g.pos[2] * g.ld[2] : 0);
+  p.dh_proj = b.f(rows * n.num_hist * 32);
+  for (int i = 0; i < 3; ++i) p.dhw[i] = b.f(i < g.nconv ? g.c[i] * g.kdim(i) : 0);
+  p.dhwl = b.f(32 * 36);
   p.bytes = b.off;
   return p;
 }
@@ -150,48 +192,63 @@ static int check_net(const DwbcNetCfg* n) {
       n->n_critic_layers < 1 || n->n_critic_layers > DWBC_MAX_LAYERS || n->n_leg_layers < 1 || n->n_leg_layers > DWBC_MAX_LAYERS ||
       n->n_arm_layers < 1 || n->n_arm_layers > DWBC_MAX_LAYERS)
     return DWBC_ERR_UNSUPPORTED;
-  // history encoder: only the tsteps == 10 variant (AC:57-62) exists for widowGo1 (WGC:124)
-  if (n->num_hist != 10 || n->hist_proj != 30 || n->hist_c1 != 20 || n->hist_k1 != 4 || n->hist_s1 != 2 || n->hist_c2 != 10 ||
-      n->hist_k2 != 2 || n->hist_s2 != 1)
-    return DWBC_ERR_UNSUPPORTED;
+  // history encoder: the conv stacks of tsteps 10, 20 and 50 (AC:52-70); the reference raises for any other tsteps
+  if (hist_variant(*n) < 0) return DWBC_ERR_UNSUPPORTED;
   if (last(n->priv_dims, n->n_priv_layers) > 32 || n->n_leg + n->n_arm > 32) return DWBC_ERR_UNSUPPORTED;
   return DWBC_OK;
 }
 
 // ---- history-encoder weight re-packing ---------------------------------------------------------
-// conv1 [20,30,4] -> W1'[20][k*32+cin]; conv2 [10,20,2] -> W2'[10][k*20+cin]; linear [L,30] over the
-// channel-major flatten (c2*3+t) -> Wl'[L][t*12+c2].  Pad entries are zero.
-__global__ void hist_pack_kernel(const float* __restrict__ w1, const float* __restrict__ w2, const float* __restrict__ wl,
-                                 float* __restrict__ o1, float* __restrict__ o2, float* __restrict__ ol, int latent) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < 20 * 128) {
-    int c1 = i / 128, r = i % 128, k = r / 32, cin = r % 32;
-    o1[i] = cin < 30 ? w1[(c1 * 30 + cin) * 4 + k] : 0.0f;
+// conv i [c,cin,k] -> Wi'[c][k*ld+cin] (ld = the row width of its input: 32, 20, 12); linear [L,30] over the channel-major flatten
+// (c*3+t) -> Wl'[L][t*12+c].  Pad entries are zero.
+struct HistPack {
+  float* w[3]; float* wp[3];      // reference-layout and re-packed conv weights (or their gradients)
+  int c[3], cin[3], k[3], ld[3];
+  int nconv;
+  float* wl; float* wlp; int latent;
+};
+static HistPack hist_pack_args(const HistGeo& g, const float* w0, const float* w1, const float* w2, const float* wl, float* const* wp, float* wlp,
+                               int latent) {
+  HistPack a{};
+  const float* w[3] = {w0, w1, w2};
+  for (int i = 0; i < g.nconv; ++i) {
+    a.w[i] = const_cast<float*>(w[i]); a.wp[i] = wp[i]; a.c[i] = g.c[i]; a.cin[i] = g.cin[i]; a.k[i] = g.k[i]; a.ld[i] = g.ld[i];
   }
-  if (i < 10 * 40) {
-    int c2 = i / 40, r = i % 40, k = r / 20, cin = r % 20;
-    o2[i] = w2[(c2 * 20 + cin) * 2 + k];
+  a.nconv = g.nconv; a.wl = const_cast<float*>(wl); a.wlp = wlp; a.latent = latent;
+  return a;
+}
+static unsigned hist_pack_grid(const HistGeo& g) {
+  int n = 32 * 36;
+  for (int i = 0; i < g.nconv; ++i) n = g.c[i] * g.kdim(i) > n ? g.c[i] * g.kdim(i) : n;
+  return (unsigned)((n + 255) / 256);
+}
+__global__ void hist_pack_kernel(const HistPack a) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  for (int l = 0; l < a.nconv; ++l) {
+    const int kd = a.k[l] * a.ld[l];
+    if (i < a.c[l] * kd) {
+      const int o = i / kd, r = i % kd, k = r / a.ld[l], cin = r % a.ld[l];
+      a.wp[l][i] = cin < a.cin[l] ? a.w[l][(o * a.cin[l] + cin) * a.k[l] + k] : 0.0f;
+    }
   }
-  if (i < latent * 36) {
+  if (i < a.latent * 36) {
     int j = i / 36, r = i % 36, t = r / 12, c2 = r % 12;
-    ol[i] = c2 < 10 ? wl[j * 30 + c2 * 3 + t] : 0.0f;
+    a.wlp[i] = c2 < 10 ? a.wl[j * 30 + c2 * 3 + t] : 0.0f;
   }
 }
-// inverse scatter of the re-packed weight gradients into the flat gradient (reference layouts)
-__global__ void hist_unpack_grad_kernel(const float* __restrict__ g1, const float* __restrict__ g2, const float* __restrict__ gl,
-                                        float* __restrict__ w1, float* __restrict__ w2, float* __restrict__ wl, int latent) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < 20 * 128) {
-    int c1 = i / 128, r = i % 128, k = r / 32, cin = r % 32;
-    if (cin < 30) w1[(c1 * 30 + cin) * 4 + k] = g1[i];
+// inverse scatter of the re-packed weight gradients (wp, wlp) into the flat gradient (w, wl: reference layouts)
+__global__ void hist_unpack_grad_kernel(const HistPack a) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  for (int l = 0; l < a.nconv; ++l) {
+    const int kd = a.k[l] * a.ld[l];
+    if (i < a.c[l] * kd) {
+      const int o = i / kd, r = i % kd, k = r / a.ld[l], cin = r % a.ld[l];
+      if (cin < a.cin[l]) a.w[l][(o * a.cin[l] + cin) * a.k[l] + k] = a.wp[l][i];
+    }
   }
-  if (i < 10 * 40) {
-    int c2 = i / 40, r = i % 40, k = r / 20, cin = r % 20;
-    w2[(c2 * 20 + cin) * 2 + k] = g2[i];
-  }
-  if (i < latent * 36) {
+  if (i < a.latent * 36) {
     int j = i / 36, r = i % 36, t = r / 12, c2 = r % 12;
-    if (c2 < 10) wl[j * 30 + c2 * 3 + t] = gl[i];
+    if (c2 < 10) a.wl[j * 30 + c2 * 3 + t] = a.wlp[i];
   }
 }
 // col2im of the conv input gradients (overlapping windows) fused with the derivative of the activation `act`:
@@ -229,20 +286,24 @@ __global__ void zero_cols_kernel(float* __restrict__ p, int64_t nrows, int ld, i
 
 static int hist_forward(const DwbcNetCfg& n, const float* P, const float* obs, const int64_t* idx, int64_t obs_stride, int rows,
                         const Plan& p, cudaStream_t st) {
+  const HistGeo g = hist_geo(n);
   const int T = n.num_hist, L = p.latent, Lld = (int)align_up(L, 4);
-  hist_pack_kernel<<<(20 * 128 + 255) / 256, 256, 0, st>>>(P + n.off_hist_w[1], P + n.off_hist_w[2], P + n.off_hist_w[3], p.hw1, p.hw2,
-                                                           p.hwl, L);
-  dwbc_launch_counter += 3;
+  hist_pack_kernel<<<hist_pack_grid(g), 256, 0, st>>>(
+      hist_pack_args(g, P + n.off_hist_w[1], P + n.off_hist_w[2], P + n.off_hist_w[3], P + n.off_hist_w[4], p.hw, p.hwl, L));
+  dwbc_launch_counter += 1 + g.nconv;
   // pad columns of the padded activation buffers are consumed by the next GEMM's K range
   zero_cols_kernel<<<(unsigned)(((int64_t)rows * T * 2 + 255) / 256), 256, 0, st>>>(p.hproj, (int64_t)rows * T, 32, 30);
-  zero_cols_kernel<<<(unsigned)(((int64_t)rows * 3 * 2 + 255) / 256), 256, 0, st>>>(p.hc2, (int64_t)rows * 3, 12, 10);
+  for (int i = 1; i < g.nconv; ++i)
+    zero_cols_kernel<<<(unsigned)(((int64_t)rows * g.pos[i + 1] * 2 + 255) / 256), 256, 0, st>>>(p.hc[i], (int64_t)rows * g.pos[i + 1], 12, 10);
   RowMat hist = rowmat_grouped(obs + (n.num_obs - T * n.num_prop), idx, T, obs_stride, n.num_prop);
   TRY(linear_fwd(hist, P + n.off_hist_w[0], n.num_prop, P + n.off_hist_b[0], p.hproj, 32, rows * T, 30, n.num_prop, mlp_act, 0, st));  // AC:80
-  RowMat a1 = rowmat_grouped(p.hproj, nullptr, 4, (int64_t)T * 32, 2 * 32);
-  TRY(linear_fwd(a1, p.hw1, 128, P + n.off_hist_b[1], p.hc1, 20, rows * 4, 20, 128, mlp_act, 0, st));                                  // AC:59
-  RowMat a2 = rowmat_grouped(p.hc1, nullptr, 3, 80, 20);
-  TRY(linear_fwd(a2, p.hw2, 40, P + n.off_hist_b[2], p.hc2, 12, rows * 3, 10, 40, mlp_act, 0, st));                                     // AC:60
-  TRY(linear_fwd(rowmat(p.hc2, 36), p.hwl, 36, P + n.off_hist_b[3], p.zh, Lld, rows, L, 36, mlp_act, 0, st));                           // AC:72
+  const float* in = p.hproj;
+  for (int i = 0; i < g.nconv; ++i) {                                                                                                   // AC:52-70
+    RowMat a = rowmat_grouped(in, nullptr, g.pos[i + 1], (int64_t)g.pos[i] * g.ld[i], g.s[i] * g.ld[i]);
+    TRY(linear_fwd(a, p.hw[i], g.kdim(i), P + n.off_hist_b[1 + i], p.hc[i], g.ld[i + 1], rows * g.pos[i + 1], g.c[i], g.kdim(i), mlp_act, 0, st));
+    in = p.hc[i];
+  }
+  TRY(linear_fwd(rowmat(in, 36), p.hwl, 36, P + n.off_hist_b[4], p.zh, Lld, rows, L, 36, mlp_act, 0, st));                              // AC:72
   return DWBC_OK;
 }
 
@@ -258,7 +319,9 @@ static int hist_latent_only(const DwbcNetCfg& n, const float* P, const float* ob
   }
   HistFusedArgs a{};
   a.wp = P + n.off_hist_w[0]; a.bp = P + n.off_hist_b[0]; a.w1 = P + n.off_hist_w[1]; a.b1 = P + n.off_hist_b[1];
-  a.w2 = P + n.off_hist_w[2]; a.b2 = P + n.off_hist_b[2]; a.wl = P + n.off_hist_w[3]; a.bl = P + n.off_hist_b[3];
+  a.w2 = P + n.off_hist_w[2]; a.b2 = P + n.off_hist_b[2]; a.wl = P + n.off_hist_w[4]; a.bl = P + n.off_hist_b[4];
+  a.variant = hist_variant(n);
+  if (n.n_hist_conv == 3) { a.w3 = P + n.off_hist_w[3]; a.b3 = P + n.off_hist_b[3]; }
   a.hist = rowmat_gather(obs + (n.num_obs - n.num_hist * n.num_prop), idx, obs_stride);
   a.out = out; a.ld_out = ld_out; a.rows = rows; a.latent = p.latent; a.act = mlp_act;
   return launch_hist_fused(a, st);
@@ -1009,43 +1072,43 @@ extern "C" int dwbc_dagger_minibatch_grad(const DwbcNetCfg* net, const float* pa
   const float* P = params;
   const int rows = M, T = n.num_hist;
   Plan p = make_plan(n, rows, workspace);
+  const HistGeo g = hist_geo(n);
   const int L = p.latent, Lld = (int)align_up(L, 4);
   if (cudaMemsetAsync(grad, 0, sizeof(float) * n.num_params, st) != cudaSuccess) return DWBC_ERR_LAUNCH;
-  if (cudaMemsetAsync(p.dhw1, 0, sizeof(float) * (20 * 128), st) != cudaSuccess) return DWBC_ERR_LAUNCH;
-  if (cudaMemsetAsync(p.dhw2, 0, sizeof(float) * (10 * 40), st) != cudaSuccess) return DWBC_ERR_LAUNCH;
+  for (int i = 0; i < g.nconv; ++i)
+    if (cudaMemsetAsync(p.dhw[i], 0, sizeof(float) * (g.c[i] * g.kdim(i)), st) != cudaSuccess) return DWBC_ERR_LAUNCH;
   if (cudaMemsetAsync(p.dhwl, 0, sizeof(float) * (32 * 36), st) != cudaSuccess) return DWBC_ERR_LAUNCH;
   TRY(priv_forward(n, P, s->observations, idx, s->obs_stride, rows, p, st));             // PPO:273-274 (no grad)
   TRY(hist_forward(n, P, s->observations, idx, s->obs_stride, rows, p, st));             // PPO:275
   dagger_loss_kernel<<<(rows + 127) / 128, 128, 0, st>>>(p.priv[n.n_priv_layers - 1], p.zh, Lld, L, p.dzh, losses_out, rows, mlp_act);
   DWBC_LAUNCH_CHECK();
-  // linear_output: zh = ELU(flat . Wl'^T + b)
+  // linear_output: zh = act(flat . Wl'^T + b)
+  const float* hlast = p.hc[g.nconv - 1];
   RowMat G4 = rowmat(p.dzh, Lld);
-  TRY(linear_bwd_weight(G4, rowmat(p.hc2, 36), p.dhwl, 36, grad + n.off_hist_b[3], rows, L, 36, st));
-  TRY(linear_bwd_data(G4, p.hwl, 36, p.d0, 36, rows, 36, L, mlp_act, rowmat(p.hc2, 36), 0, st));    // d(conv2 pre-act) as [rows*3, 12]
-  // conv2
-  RowMat G3 = rowmat(p.d0, 12);
-  TRY(linear_bwd_weight(G3, rowmat_grouped(p.hc1, nullptr, 3, 80, 20), p.dhw2, 40, grad + n.off_hist_b[2], rows * 3, 10, 40, st));
-  TRY(linear_bwd_data(G3, p.hw2, 40, p.dh_a2, 40, rows * 3, 40, 10, ACT_NONE, RowMat{}, 0, st));
-  {
-    int64_t tot = (int64_t)rows * 4 * 20;
-    col2im_dact_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(p.dh_a2, p.hc1, p.dh_c1, rows, 4, 20, 20, 3, 2, 1, mlp_act);
+  TRY(linear_bwd_weight(G4, rowmat(hlast, 36), p.dhwl, 36, grad + n.off_hist_b[4], rows, L, 36, st));
+  TRY(linear_bwd_data(G4, p.hwl, 36, p.d0, 36, rows, 36, L, mlp_act, rowmat(hlast, 36), 0, st));    // d(last conv pre-act) as [rows*3, 12]
+  // convs, last first: weight gradient, im2col-space input gradient, then col2im with the input's activation derivative
+  const float* gout = p.d0;
+  for (int i = g.nconv - 1; i >= 0; --i) {
+    const float* in = i == 0 ? p.hproj : p.hc[i - 1];
+    float* dst = i == 0 ? p.dh_proj : p.dh_c[i - 1];
+    const int rows_o = rows * g.pos[i + 1], kd = g.kdim(i);
+    RowMat G = rowmat(gout, g.ld[i + 1]);
+    TRY(linear_bwd_weight(G, rowmat_grouped(in, nullptr, g.pos[i + 1], (int64_t)g.pos[i] * g.ld[i], g.s[i] * g.ld[i]), p.dhw[i], kd,
+                          grad + n.off_hist_b[1 + i], rows_o, g.c[i], kd, st));
+    TRY(linear_bwd_data(G, p.hw[i], kd, p.dh_a[i], kd, rows_o, kd, g.c[i], ACT_NONE, RowMat{}, 0, st));
+    int64_t tot = (int64_t)rows * g.pos[i] * g.ld[i];
+    col2im_dact_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(p.dh_a[i], in, dst, rows, g.pos[i], g.cin[i], g.ld[i], g.pos[i + 1], g.k[i],
+                                                                     g.s[i], mlp_act);
     DWBC_LAUNCH_CHECK();
-  }
-  // conv1
-  RowMat G2 = rowmat(p.dh_c1, 20);
-  TRY(linear_bwd_weight(G2, rowmat_grouped(p.hproj, nullptr, 4, (int64_t)T * 32, 64), p.dhw1, 128, grad + n.off_hist_b[1], rows * 4, 20, 128, st));
-  TRY(linear_bwd_data(G2, p.hw1, 128, p.dh_a1, 128, rows * 4, 128, 20, ACT_NONE, RowMat{}, 0, st));
-  {
-    int64_t tot = (int64_t)rows * T * 32;
-    col2im_dact_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(p.dh_a1, p.hproj, p.dh_proj, rows, T, 30, 32, 4, 4, 2, mlp_act);
-    DWBC_LAUNCH_CHECK();
+    gout = dst;
   }
   // projection
   RowMat G1 = rowmat(p.dh_proj, 32);
   RowMat hist = rowmat_grouped(s->observations + (n.num_obs - T * n.num_prop), idx, T, s->obs_stride, n.num_prop);
   TRY(linear_bwd_weight(G1, hist, grad + n.off_hist_w[0], n.num_prop, grad + n.off_hist_b[0], rows * T, 30, n.num_prop, st));
-  hist_unpack_grad_kernel<<<(20 * 128 + 255) / 256, 256, 0, st>>>(p.dhw1, p.dhw2, p.dhwl, grad + n.off_hist_w[1], grad + n.off_hist_w[2],
-                                                                   grad + n.off_hist_w[3], L);
+  hist_unpack_grad_kernel<<<hist_pack_grid(g), 256, 0, st>>>(
+      hist_pack_args(g, grad + n.off_hist_w[1], grad + n.off_hist_w[2], grad + n.off_hist_w[3], grad + n.off_hist_w[4], p.dhw, p.dhwl, L));
   DWBC_LAUNCH_CHECK();
   return DWBC_OK;
 }

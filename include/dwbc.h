@@ -33,7 +33,7 @@ enum {
   DWBC_ERR_LAUNCH = -3       /* cudaGetLastError() != cudaSuccess after the launch */
 };
 
-#define DWBC_ABI_VERSION 4
+#define DWBC_ABI_VERSION 5
 #define DWBC_MAX_DOF 24
 #define DWBC_MAX_TERMS 40   /* active reward terms per channel */
 #define DWBC_MAX_IDX 8      /* penalised / termination contact bodies */
@@ -187,7 +187,8 @@ typedef struct DwbcStepArgs {
   float leg_termination_scale, arm_termination_scale;                  /* 0 when inactive */
   int32_t generic_kernel;        /* 1 = always run the warp-per-env kernel (any N; only obs_buf and obs_history must be 16-B aligned),
                                     0 = pick by shape: the 16-envs-per-CTA TMA kernel when N is a multiple of 32 and every row block
-                                    is 16-B aligned, else the warp-per-env kernel */
+                                    is 16-B aligned (and history_len == 10, num_prop == 76: the shapes it is specialised to), else the
+                                    warp-per-env kernel, which streams history rows longer than 1024 floats instead of holding them */
   int32_t reserved_;
 } DwbcStepArgs;
 
@@ -258,11 +259,18 @@ typedef struct DwbcNetCfg {
   int32_t n_critic_layers, critic_dims[DWBC_MAX_LAYERS];
   int32_t n_leg_layers, leg_dims[DWBC_MAX_LAYERS];   /* hidden dims of the leg heads (actor and critic) */
   int32_t n_arm_layers, arm_dims[DWBC_MAX_LAYERS];
-  int32_t hist_proj, hist_c1, hist_k1, hist_s1, hist_c2, hist_k2, hist_s2; /* AC:49-62 (tsteps==10: 30,20,4,2,10,2,1) */
+  /* StateHistoryEncoder geometry (AC:49-73), one row per tsteps = num_hist; any other combination is DWBC_ERR_UNSUPPORTED:
+   *   num_hist  proj  c1 k1 s1   c2 k2 s2   c3 k3 s3   n_hist_conv   conv positions
+   *      10      30   20  4  2   10  2  1    0  0  0        2        10 -> 4 -> 3
+   *      20      30   20  6  2   10  4  2    0  0  0        2        20 -> 8 -> 3
+   *      50      30   20  8  4   10  5  1   10  5  1        3        50 -> 11 -> 7 -> 3
+   * Every variant ends at 3 positions x 10 channels, the 30 inputs of linear_output (channel-major flatten c * 3 + t). */
+  int32_t hist_proj, hist_c1, hist_k1, hist_s1, hist_c2, hist_k2, hist_s2;
+  int32_t hist_c3, hist_k3, hist_s3, n_hist_conv;
   int64_t num_params;
   int64_t off_std;
   int64_t off_priv_w[DWBC_MAX_LAYERS], off_priv_b[DWBC_MAX_LAYERS];
-  int64_t off_hist_w[4], off_hist_b[4];              /* encoder.0, conv_layers.0, conv_layers.2, linear_output.0 */
+  int64_t off_hist_w[5], off_hist_b[5];              /* encoder.0, conv_layers.0, conv_layers.2, conv_layers.4 (n_hist_conv == 3 only), linear_output.0 */
   int64_t off_actor_w[DWBC_MAX_LAYERS], off_actor_b[DWBC_MAX_LAYERS];
   int64_t off_aleg_w[DWBC_MAX_LAYERS + 1], off_aleg_b[DWBC_MAX_LAYERS + 1];
   int64_t off_aarm_w[DWBC_MAX_LAYERS + 1], off_aarm_b[DWBC_MAX_LAYERS + 1];
