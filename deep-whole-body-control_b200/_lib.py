@@ -15,6 +15,8 @@ LIB_PATH = os.path.join(_HERE, "libdwbc.so")
 ABI_VERSION = 5
 MAX_DOF, MAX_TERMS, MAX_IDX, MAX_SLOTS, NUM_METRICS, RAND_COLS, MAX_LAYERS = 24, 40, 8, 64, 10, 104, 4
 GS, DS = 28, 72
+# device scratch sizes (dwbc.h): dwbc_clip_adam_step norm partials, dwbc_gae stats (doubles)
+NORM_SCRATCH, GAE_STATS = 592, 4 + 2 * 1024
 GS_COL = dict(commands=0, goal_timer=3, traj_timesteps=4, traj_total_timesteps=5, ee_start_sphere=6, ee_goal_sphere=9,
               ee_goal_cart=12, curr_ee_goal_sphere=15, curr_ee_goal_cart=18, ee_goal_delta_orn_euler=21, ee_goal_orn_euler=24)
 DS_COL = dict(base_lin_vel=0, base_ang_vel=3, base_yaw_euler=6, base_yaw_quat=9, last_root_vel=13, feet_air_time=19,
@@ -63,7 +65,7 @@ class EnvBuffers(C.Structure):
         "action_history", "mass_params", "friction", "motor_strength", "env_origins", "box_env_origins_delta_y",
         "goal_state", "derived_state", "episode_length", "obs_history", "episode_sums", "height_samples",
         "measured_heights", "heights_obs", "terrain_levels", "terrain_types", "terrain_origins", "obs_buf")] + \
-        [("obs_stride", i64)] + [(n, vp) for n in ("rew_buf", "arm_rew_buf", "reset_buf", "time_out_buf", "episode_stats",
+        [("obs_stride", i64)] + [(n, vp) for n in ("rew_buf", "arm_rew_buf", "reset_buf", "time_out_buf", "episode_stats", "episode_scratch",
                                                    "store_values", "store_rewards", "store_dones")] + [("store_gamma", f32), ("reserved_", i32)]
 
 

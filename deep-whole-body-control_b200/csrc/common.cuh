@@ -78,4 +78,20 @@ __device__ __forceinline__ float philox_uniform(uint64_t seed, uint64_t step, in
   return u01(x);
 }
 
+// Fixed-order sums across blocks: every block writes its partials to a slot of its own, then calls this.  It returns true, in every
+// thread, in the block that arrives last (counted on `ticket`, which that block returns to zero for the next launch); that block sees
+// every partial and adds them up in slot order, so the result does not depend on which block ran when.
+__device__ __forceinline__ bool last_block(unsigned* ticket) {
+  __shared__ bool last;
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    last = atomicAdd(ticket, 1u) == gridDim.x * gridDim.y * gridDim.z - 1;
+    if (last) *ticket = 0u;
+  }
+  __syncthreads();
+  if (last) __threadfence();
+  return last;
+}
+
 }  // namespace dwbc

@@ -494,12 +494,11 @@ env_step_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant__ 
       hist_zeroed = true;
     }
     ep = 0;
-    // extras['episode'] means (WG:743-750): sum over reset envs via atomics, divided on the host
+    // extras['episode'] means (WG:743-750): the ended episode's sums go to this env's slot; episode_stats_kernel adds them up
     for (int i = lane; i < nslots; i += 32) {
-      atomicAdd(B.episode_stats + 1 + i, sm[S_SUM + i]);
+      B.episode_scratch[(size_t)e * cfg.sums_stride + i] = sm[S_SUM + i];
       sm[S_SUM + i] = 0.0f;
     }
-    if (lane == 0) atomicAdd(B.episode_stats, 1.0f);
     __syncwarp();
   }
   if (root_dirty && lane < 13) root_g[lane] = sm[S_ROOT + lane];
@@ -640,6 +639,31 @@ int dwbc_launch_env_step_v2(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, co
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
+// extras['episode'] of one step in a fixed order: block c adds column c of the slots of the envs that reset, in env order (thread t:
+// envs t, t + 256, ...; then a fixed tree), column 0 counting them; episode_stats[c] += that sum
+__global__ void __launch_bounds__(256) episode_stats_kernel(const uint8_t* __restrict__ reset, const float* __restrict__ slots, int stride, int n,
+                                                            float* __restrict__ stats) {
+  __shared__ float red[256];
+  const int c = blockIdx.x;
+  float s = 0.0f;
+  for (int e = threadIdx.x; e < n; e += 256)
+    if (reset[e]) s += c == 0 ? 1.0f : slots[(size_t)e * stride + c - 1];
+  red[threadIdx.x] = s;
+  __syncthreads();
+  for (int w = 128; w > 0; w >>= 1) {
+    if ((int)threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) stats[c] += red[0];
+}
+
+static int launch_episode_stats(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, cudaStream_t st) {
+  episode_stats_kernel<<<1 + cfg->n_sum_slots + DWBC_NUM_METRICS, 256, 0, st>>>(buf->reset_buf, buf->episode_scratch, cfg->sums_stride,
+                                                                              cfg->num_envs, buf->episode_stats);
+  DWBC_LAUNCH_CHECK();
+  return DWBC_OK;
+}
+
 extern "C" int dwbc_post_physics_step(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, const DwbcStepArgs* args,
                                       dwbc_stream_t stream) {
   if (!cfg || !buf || !args) return DWBC_ERR_ARG;
@@ -661,7 +685,7 @@ extern "C" int dwbc_post_physics_step(const DwbcEnvCfg* cfg, const DwbcEnvBuffer
       !buf->torques || !buf->actions || !buf->action_history || !buf->mass_params || !buf->friction || !buf->motor_strength ||
       !buf->env_origins || !buf->box_env_origins_delta_y || !buf->goal_state || !buf->derived_state || !buf->episode_length ||
       !buf->obs_history || !buf->episode_sums || !buf->obs_buf || !buf->rew_buf || !buf->arm_rew_buf || !buf->reset_buf ||
-      !buf->time_out_buf || !buf->episode_stats || (buf->store_rewards && !buf->store_values))
+      !buf->time_out_buf || !buf->episode_stats || !buf->episode_scratch || (buf->store_rewards && !buf->store_values))
     return DWBC_ERR_ARG;
   // both kernels move observation rows and history rows in 16-byte vectors
   if (!aligned16(buf->obs_buf) || !aligned16(buf->obs_history)) return DWBC_ERR_UNSUPPORTED;
@@ -670,8 +694,8 @@ extern "C" int dwbc_post_physics_step(const DwbcEnvCfg* cfg, const DwbcEnvBuffer
       aligned16(buf->torques) && aligned16(buf->actions) && aligned16(buf->action_history) && aligned16(buf->mass_params) &&
       aligned16(buf->friction) && aligned16(buf->motor_strength) && aligned16(buf->goal_state) && aligned16(buf->derived_state) &&
       aligned16(buf->episode_length) && aligned16(buf->episode_sums) && !args->generic_kernel) {
-    int rc = dwbc_launch_env_step_v2(cfg, buf, args, (cudaStream_t)stream);
-    if (rc != DWBC_ERR_UNSUPPORTED) return rc;
+    const int rc = dwbc_launch_env_step_v2(cfg, buf, args, (cudaStream_t)stream);
+    if (rc != DWBC_ERR_UNSUPPORTED) return rc == DWBC_OK ? launch_episode_stats(cfg, buf, (cudaStream_t)stream) : rc;
   }
   const int grid = (cfg->num_envs + ENV_WARPS - 1) / ENV_WARPS;
   if ((int64_t)cfg->history_len * cfg->num_prop <= MAX_H4 * 128)
@@ -679,7 +703,7 @@ extern "C" int dwbc_post_physics_step(const DwbcEnvCfg* cfg, const DwbcEnvBuffer
   else
     env_step_kernel<true><<<grid, ENV_WARPS * 32, 0, (cudaStream_t)stream>>>(*cfg, *buf, *args);
   DWBC_LAUNCH_CHECK();
-  return DWBC_OK;
+  return launch_episode_stats(cfg, buf, (cudaStream_t)stream);
 }
 
 extern "C" int dwbc_fill_uniform(float* out, int32_t num_envs, uint64_t seed, uint64_t step, dwbc_stream_t stream) {

@@ -701,14 +701,11 @@ env_step_v2_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant
       if (lane < 4) ds[DWBC_DS_FEET_AIR_TIME + lane] = 0.0f;
       float* ah = sm + Ly::o_ah + e * AH * NA;
       for (int i = lane; i < AH * NA; i += 32) ah[i] = 0.0f;
-      for (int i = lane; i < nslots; i += 32) {  // extras['episode'] (WG:743-750)
-        atomicAdd(B.episode_stats + 1 + i, sums[i]);
+      for (int i = lane; i < nslots; i += 32) {  // extras['episode'] (WG:743-750): this env's slot, added up by episode_stats_kernel
+        B.episode_scratch[(size_t)env * cfg.sums_stride + i] = sums[i];
         sums[i] = 0.0f;
       }
-      if (lane == 0) {
-        atomicAdd(B.episode_stats, 1.0f);
-        flags_s[e] = flags | F_FILL | F_ROOT_DIRTY | F_DOF_DIRTY;
-      }
+      if (lane == 0) flags_s[e] = flags | F_FILL | F_ROOT_DIRTY | F_DOF_DIRTY;
     }
   }
   cbar();

@@ -14,7 +14,11 @@ namespace dwbc {
 
 constexpr int GAE_BLOCK = 64;
 
-__device__ __forceinline__ void block_accumulate(double s, double ss, double* stats) {
+// stats layout (DWBC_GAE_STATS doubles): [0..2] = (n, sum, sum of squares), [3] = counter, [4 + 2 b, 4 + 2 b + 1] = partials of block b
+constexpr int GAE_PART = 4;
+
+// this block's (sum, sum of squares) -> its own slot
+__device__ __forceinline__ void block_partial(double s, double ss, double* stats) {
   __shared__ double red[2][GAE_BLOCK / 32];
   s = warp_sum(s);
   ss = warp_sum(ss);
@@ -24,9 +28,27 @@ __device__ __forceinline__ void block_accumulate(double s, double ss, double* st
   if (threadIdx.x == 0) {
     double a = 0, b = 0;
     for (int i = 0; i < GAE_BLOCK / 32; ++i) { a += red[0][i]; b += red[1][i]; }
-    atomicAdd(stats + 1, a);
-    atomicAdd(stats + 2, b);
+    stats[GAE_PART + 2 * blockIdx.x] = a;
+    stats[GAE_PART + 2 * blockIdx.x + 1] = b;
   }
+}
+// The partials of all blocks added up in block order (thread t: blocks t, t + 64, ...; then a fixed tree), the same in every block
+__device__ __forceinline__ double2 sum_partials(const double* stats) {
+  __shared__ double red[2][GAE_BLOCK];
+  double a = 0.0, b = 0.0;
+  for (int i = threadIdx.x; i < (int)gridDim.x; i += GAE_BLOCK) {
+    a += __ldcg(stats + GAE_PART + 2 * i);
+    b += __ldcg(stats + GAE_PART + 2 * i + 1);
+  }
+  red[0][threadIdx.x] = a;
+  red[1][threadIdx.x] = b;
+  __syncthreads();
+#pragma unroll
+  for (int w = GAE_BLOCK / 2; w > 0; w >>= 1) {
+    if ((int)threadIdx.x < w) { red[0][threadIdx.x] += red[0][threadIdx.x + w]; red[1][threadIdx.x] += red[1][threadIdx.x + w]; }
+    __syncthreads();
+  }
+  return make_double2(red[0][0], red[1][0]);
 }
 
 template <bool kFused>
@@ -56,19 +78,23 @@ gae_kernel(const float* __restrict__ rewards, const float* __restrict__ values, 
       nxt = v;
     }
   }
-  block_accumulate(s, ss, stats);
-  if (threadIdx.x == 0 && blockIdx.x == 0) atomicAdd(stats, (double)T * (double)C);
+  block_partial(s, ss, stats);
+  const double n = (double)T * (double)C;
   if constexpr (kFused) {
     __threadfence();
     cg::this_grid().sync();
-    const double n = (double)T * (double)C;
-    const double sum = __ldcg(stats + 1), sq = __ldcg(stats + 2);
-    const double mean = sum / n;
-    const double var = fmax((sq - sum * sum / n) / (n - 1.0), 0.0);
+    const double2 tot = sum_partials(stats);
+    if (threadIdx.x == 0 && blockIdx.x == 0) { stats[0] += n; stats[1] += tot.x; stats[2] += tot.y; }
+    const double mean = tot.x / n;
+    const double var = fmax((tot.y - tot.x * tot.x / n) / (n - 1.0), 0.0);
     const float fm = (float)mean, fd = (float)sqrt(var) + 1e-8f;  // RS:150
     const size_t total = (size_t)T * C;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x)
       advantages[i] = (__ldcg(advantages + i) - fm) / fd;
+  } else {
+    if (!last_block(reinterpret_cast<unsigned*>(stats + 3))) return;
+    const double2 tot = sum_partials(stats);
+    if (threadIdx.x == 0) { stats[0] += n; stats[1] += tot.x; stats[2] += tot.y; }
   }
 }
 
@@ -103,6 +129,7 @@ extern "C" int dwbc_gae(const float* rewards, const float* values, const uint8_t
   if (!rewards || !values || !dones || !last_values || !returns || !advantages || !stats || T <= 0 || N <= 0) return DWBC_ERR_ARG;
   const int C = 2 * N;
   int grid = (C + GAE_BLOCK - 1) / GAE_BLOCK;
+  if (grid > DWBC_GAE_MAX_BLOCKS) grid = DWBC_GAE_MAX_BLOCKS;   // one partial slot per block; grid-stride loops cover the rest
   cudaStream_t st = (cudaStream_t)stream;
   if (normalize && (size_t)T * C > 1) {
     int dev = 0, sms = 0, per_sm = 0;

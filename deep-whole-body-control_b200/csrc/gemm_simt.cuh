@@ -3,7 +3,7 @@
 //
 //   FWD      Y[m,n]  = act( beta*Y + sum_k X[m,k] * W[n,k] + b[n] )            (nn.Linear fwd)
 //   BWD_DATA dX[m,n] = ( beta*dX + sum_k G[m,k] * W[k,n] ) * act'(Xact[m,n])   (dgrad, fused act')
-//   BWD_WGT  dW[m,n] += sum_k G[k,m] * X[k,n];  db[m] += sum_k G[k,m]          (wgrad, split-K + atomics)
+//   BWD_WGT  dW[m,n] += sum_k G[k,m] * X[k,n];  db[m] += sum_k G[k,m]          (wgrad, split-K, fixed-order sum of the splits)
 //
 // Matrices that are indexed by a *row* (activations, the rollout storage) are described by a
 // RowMat, which can gather rows through an index vector (mini-batch gather, RS:189-201, without
@@ -90,7 +90,64 @@ struct GemmArgs {
   int beta;             // 0/1: accumulate onto C (FWD, BWD_DATA)
   int M, N, K;          // C is M x N, reduction length K
   int k_chunk;          // BWD_WGT: reduction rows per CTA (split-K)
+  float* part;          // BWD_WGT: split z writes its [M x N] partial at part + z M N, its bias partial at part + splits M N + z M
 };
+
+// ---- fixed-order sums of partials ---------------------------------------------------------------------------------------------
+// Split-K GEMMs and the grouped weight-gradient launch leave one partial per (output, slab of rows); this pass adds them up in slab order
+// and adds the result to the output: dst[r * ld + c] += sum_s part[off + s * stride + r * cols + c], s = 0 .. nslab - 1.
+constexpr int RED_MAX = 40;
+struct RedTarget { float* dst; int64_t ld, off, stride, first; int rows, cols, nslab; };
+struct RedArgs { const float* part; int n; int64_t total; RedTarget t[RED_MAX]; };
+
+__global__ void __launch_bounds__(256) partials_reduce_kernel(const __grid_constant__ RedArgs a) {
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < a.total; e += (int64_t)gridDim.x * blockDim.x) {
+    int i = 0;
+    while (i + 1 < a.n && e >= a.t[i + 1].first) ++i;
+    const RedTarget& t = a.t[i];
+    const int64_t k = e - t.first, r = k / t.cols, c = k - r * t.cols;
+    const float* p = a.part + t.off + k;
+    float s = 0.0f;
+#pragma unroll 4
+    for (int j = 0; j < t.nslab; ++j) s += __ldcg(p + (int64_t)j * t.stride);
+    t.dst[r * t.ld + c] += s;
+  }
+}
+struct RedBuilder {
+  RedArgs a{};
+  void add(float* dst, int64_t ld, int rows, int cols, int64_t off, int64_t stride, int nslab) {
+    a.t[a.n] = RedTarget{dst, ld, off, stride, a.total, rows, cols, nslab};
+    a.total += (int64_t)rows * cols;
+    ++a.n;
+  }
+  int launch(const float* part, cudaStream_t st) {
+    a.part = part;
+    int64_t grid = (a.total + 255) / 256;
+    if (grid > 1184) grid = 1184;
+    partials_reduce_kernel<<<(unsigned)grid, 256, 0, st>>>(a);
+    ++dwbc_launch_counter;
+    return cudaGetLastError() == cudaSuccess ? DWBC_OK : DWBC_ERR_LAUNCH;
+  }
+};
+
+// Scratch of the weight-gradient partials, set by the entry point that launches them (the update workspace, or stream-ordered memory
+// of a debug entry point): the launches fail with DWBC_ERR_ARG rather than write past `mlp_wpart_cap` floats.
+extern thread_local float* mlp_wpart;
+extern thread_local int64_t mlp_wpart_cap;
+
+// splits of a split-K weight gradient (about 4 CTAs per SM over the grid, at least 64 rows per split); the CTAs times the splits stay
+// below tiles + 592, which bounds the partials
+inline int simt_wgrad_chunk(int M, int N, int K) {
+  const int tiles = ((M + GT_M - 1) / GT_M) * ((N + GT_N - 1) / GT_N);
+  const int splits = (592 + tiles - 1) / tiles;
+  int chunk = (K + splits - 1) / splits;
+  chunk = ((chunk + GT_K - 1) / GT_K) * GT_K;
+  return chunk < 64 ? 64 : chunk;
+}
+inline int64_t simt_wgrad_floats(int M, int N, int K) {
+  const int64_t splits = (K + simt_wgrad_chunk(M, N, K) - 1) / simt_wgrad_chunk(M, N, K);
+  return splits * ((int64_t)M * N + M);
+}
 
 // tile loaders: S is [GT_K][GT_M + GT_PAD]
 // (a) rows of the RowMat run along the tile's M/N axis, columns along K  -> transposed store
@@ -183,6 +240,7 @@ __global__ void __launch_bounds__(GT_THREADS) gemm_tile_kernel(const GemmArgs g)
 
   // ---- epilogue ----
   if (kMode == GEMM_BWD_WGT) {
+    float* P = g.part + (int64_t)blockIdx.z * g.M * g.N;      // this split's slot
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const int m = m0 + ty * 4 + i;
@@ -190,7 +248,7 @@ __global__ void __launch_bounds__(GT_THREADS) gemm_tile_kernel(const GemmArgs g)
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const int n = n0 + tx * 4 + j;
-        if (n < g.N) atomicAdd(g.C + (int64_t)m * g.ldc + n, acc[i][j]);
+        if (n < g.N) P[(int64_t)m * g.N + n] = acc[i][j];
       }
     }
     if (g.dbias && blockIdx.y == 0) {
@@ -202,7 +260,8 @@ __global__ void __launch_bounds__(GT_THREADS) gemm_tile_kernel(const GemmArgs g)
         for (int k = k_begin + q; k < k_end; k += 4) s += g.A.row(k)[m0 + col];
       part[q][col] = s;
       __syncthreads();
-      if (q == 0 && m0 + col < g.M) atomicAdd(g.dbias + m0 + col, (part[0][col] + part[1][col]) + (part[2][col] + part[3][col]));
+      if (q == 0 && m0 + col < g.M)
+        g.part[(int64_t)gridDim.z * g.M * g.N + (int64_t)blockIdx.z * g.M + m0 + col] = (part[0][col] + part[1][col]) + (part[2][col] + part[3][col]);
     }
     return;
   } else {
@@ -238,14 +297,22 @@ template <int kMode>
 inline int launch_gemm(const GemmArgs& g, cudaStream_t st) {
   if (g.M <= 0 || g.N <= 0 || g.K <= 0) return DWBC_ERR_ARG;
   dim3 grid((g.M + GT_M - 1) / GT_M, (g.N + GT_N - 1) / GT_N, 1);
-  if (kMode == GEMM_BWD_WGT) grid.z = (g.K + g.k_chunk - 1) / g.k_chunk;
+  if (kMode == GEMM_BWD_WGT) {
+    grid.z = (g.K + g.k_chunk - 1) / g.k_chunk;
+    if (!g.part || (int64_t)grid.z * ((int64_t)g.M * g.N + g.M) > mlp_wpart_cap) return DWBC_ERR_ARG;
+  }
   const bool va = rowmat_vec_ok(g.A), vb = rowmat_vec_ok(g.B);
   if (va && vb) gemm_tile_kernel<kMode, true, true><<<grid, GT_THREADS, 0, st>>>(g);
   else if (va) gemm_tile_kernel<kMode, true, false><<<grid, GT_THREADS, 0, st>>>(g);
   else if (vb) gemm_tile_kernel<kMode, false, true><<<grid, GT_THREADS, 0, st>>>(g);
   else gemm_tile_kernel<kMode, false, false><<<grid, GT_THREADS, 0, st>>>(g);
   ++dwbc_launch_counter;
-  return cudaGetLastError() == cudaSuccess ? DWBC_OK : DWBC_ERR_LAUNCH;
+  if (cudaGetLastError() != cudaSuccess) return DWBC_ERR_LAUNCH;
+  if (kMode != GEMM_BWD_WGT) return DWBC_OK;
+  RedBuilder r;                                    // the splits in split order
+  r.add(g.C, g.ldc, g.M, g.N, 0, (int64_t)g.M * g.N, (int)grid.z);
+  if (g.dbias) r.add(g.dbias, 0, 1, g.M, (int64_t)grid.z * g.M * g.N, g.M, (int)grid.z);
+  return r.launch(g.part, st);
 }
 
 }  // namespace dwbc

@@ -344,12 +344,8 @@ inline int linear_bwd_data(RowMat G, const float* W, int64_t ldw, float* dX, int
 inline int linear_bwd_weight(RowMat G, RowMat X, float* dW, int64_t lddw, float* db, int rows, int Nout, int Nin, cudaStream_t st) {
   GemmArgs g{};
   g.A = G; g.B = X; g.C = dW; g.ldc = lddw; g.dbias = db; g.M = Nout; g.N = Nin; g.K = rows;
-  int tiles = ((Nout + GT_M - 1) / GT_M) * ((Nin + GT_N - 1) / GT_N);
-  int splits = (592 + tiles - 1) / tiles;                 // ~4 CTAs per SM over the whole grid
-  int chunk = (rows + splits - 1) / splits;
-  chunk = ((chunk + GT_K - 1) / GT_K) * GT_K;
-  if (chunk < 64) chunk = 64;
-  g.k_chunk = chunk;
+  g.k_chunk = simt_wgrad_chunk(Nout, Nin, rows);
+  g.part = mlp_wpart;
   return dispatch_gemm<GEMM_BWD_WGT>(g, st);
 }
 

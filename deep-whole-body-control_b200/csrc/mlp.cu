@@ -23,6 +23,9 @@ thread_local int mlp_precision = 0;
 // hidden-layer activation of the CURRENT call (DwbcNetCfg.activation as an ACT_* code, set by every entry point): every layer of the
 // encoders, backbones and head hidden layers; the actor heads' outputs keep tanh and the critic heads' stay linear
 thread_local int mlp_act = 0;
+// partial area of the weight-gradient launches of the CURRENT call (gemm_simt.cuh): the workspace's, set by make_plan
+thread_local float* mlp_wpart = nullptr;
+thread_local int64_t mlp_wpart_cap = 0;
 int tc_debug = 0;
 
 static inline int64_t align_up(int64_t x, int64_t a) { return (x + a - 1) / a * a; }
@@ -57,7 +60,10 @@ struct Plan {
   float* zh;                      // [rows, latent]
   float* hw[3]; float* hwl;                // re-packed weights: conv i [c_i][k_i*ld[i]], linear_output [32][36]
   float* wpack;                            // packed weight images of the fused chain kernels (mlp_chain2.cuh)
-  int* queue;                              // work-item counters of the chain kernel (zero between launches)
+  int* queue;                              // counters, zero between launches: [0..1] work queue of the chain kernel, [2] ppo_loss_kernel, [3]
+                                           // dagger_loss_kernel
+  float* loss_part;                        // per-block / per-(tile, warp) partial sums of the loss kernels
+  float* wpart;                            // per-(GEMM, slab) / per-(split) partials of the weight gradients (wpart_floats)
   // gradients
   float* g_leg; float* g_arm; float* g_vl; float* g_va; float* g_z;   // g_vl / g_va: columns 0 / 1 of one [rows, 4] buffer
   // per-layer pre-activation gradients kept by the fused backward chain for the weight-gradient GEMMs
@@ -124,6 +130,26 @@ static inline bool img_dim(int d) { return d == 128; }
 static inline int64_t act_floats(int64_t rows, int d) { return img_dim(d) ? align_up(rows, 128) * 128 : rows * align_up(d, 4); }
 static inline RowMat act_mat(const float* p, int d) { return img_dim(d) ? rowmat_image(p) : rowmat(p, d); }
 
+constexpr int LOSS_PART = 40;              // ppo_loss_kernel, per block: the five loss means, then the std gradient (<= 32)
+// partial sums of the loss hooks: one slot per (128-row tile, worker warp) of the chain kernel, one per 128-row block of ppo_loss_kernel
+static int64_t loss_part_floats(int64_t rows) {
+  static_assert(C2_FIN_PART >= LOSS_PART, "one area serves both");
+  return (rows + 127) / 128 * C2_WORKERS * C2_FIN_PART;
+}
+
+// Partials of the weight-gradient launches, for every plan a call with `rows` rows can make (any SM count, any dwbc_debug_set_wgrad_items),
+// and never fewer for more rows: the largest of
+//   the grouped launch: at most wg_max_nslab(rows) slabs per GEMM, and its GEMMs' slots hold at most every parameter (+ alignment);
+//   one layer-wise TF32 weight gradient (<= 128 x 128) over at most rows x num_hist rows (the history projection);
+//   one split-K CUDA-core weight gradient: CTAs x splits < tiles + 592, tiles <= (d / 64)^2 for the widest operand d.
+static int64_t wpart_floats(const DwbcNetCfg& n, int64_t rows) {
+  const int64_t group = wg_max_nslab(rows) * (n.num_params + 4 * WG_MAX);
+  const int64_t one = wg_max_nslab(rows * n.num_hist) * wg_slot(128, 128);
+  const int64_t d = std::max<int64_t>(maxdim(n), std::max(n.num_prop + n.num_priv, 256)), t = ((d + 63) / 64) * ((d + 63) / 64);
+  const int64_t simt = (t + 592) * (GT_M * GT_N + GT_M);
+  return std::max(group, std::max(one, simt));
+}
+
 static Plan make_plan(const DwbcNetCfg& n, int64_t rows, void* ws) {
   Plan p{};
   Bump b{reinterpret_cast<char*>(ws), 0};
@@ -166,7 +192,10 @@ static Plan make_plan(const DwbcNetCfg& n, int64_t rows, void* ws) {
   p.dh_proj = b.f(rows * n.num_hist * 32);
   for (int i = 0; i < 3; ++i) p.dhw[i] = b.f(i < g.nconv ? g.c[i] * g.kdim(i) : 0);
   p.dhwl = b.f(32 * 36);
+  p.loss_part = b.f(loss_part_floats(rows));
+  p.wpart = b.f(wpart_floats(n, rows));
   p.bytes = b.off;
+  if (ws) { mlp_wpart = p.wpart; mlp_wpart_cap = wpart_floats(n, rows); }     // (the area the weight-gradient launches of this call use)
   return p;
 }
 
@@ -527,6 +556,7 @@ struct LossArgs {
   const float* actions; const float* old_logp; const float* old_values; const float* returns; const float* adv; const int64_t* idx;
   float* g_leg; int gleg_ld; float* g_arm; int garm_ld; float* g_vl; float* g_va; int gv_ld; float* g_z;
   float* grad_std; float* losses;
+  float* part; unsigned* ticket;          // [blocks][LOSS_PART] partials, added up in block order by the last block
   int rows, n_leg, n_act, latent;
   float clip, c_value, c_ent, c_reg, rho;
   int clipped_value;
@@ -534,8 +564,7 @@ struct LossArgs {
 };
 
 __global__ void __launch_bounds__(128) ppo_loss_kernel(const LossArgs a) {
-  __shared__ float red[5][4];
-  __shared__ float sred[32];
+  __shared__ float red[5 + 32][4];
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   const bool on = r < a.rows;
   const float inv2m = 1.0f / (2.0f * (float)a.rows), invm = 1.0f / (float)a.rows;
@@ -630,7 +659,7 @@ __global__ void __launch_bounds__(128) ppo_loss_kernel(const LossArgs a) {
     for (int i = 0; i < a.latent; ++i)
       a.g_z[(int64_t)r * a.zld + i] = s * (a.zp[(int64_t)r * a.zld + i] - zhr[i]);
   }
-  // block reductions -> one atomic per CTA per quantity
+  // warp sums -> this block's slot; the last block adds the slots up in block order
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   float v4[5] = {l_surr * inv2m, l_val * inv2m, l_reg * invm, l_ent * inv2m, l_ts * invm / (float)max(a.n_act - a.n_leg, 1)};
 #pragma unroll
@@ -638,23 +667,27 @@ __global__ void __launch_bounds__(128) ppo_loss_kernel(const LossArgs a) {
     float s = warp_sum(v4[k]);
     if (lane == 0) red[k][w] = s;
   }
-  if (threadIdx.x < 32) sred[threadIdx.x] = 0.0f;
-  __syncthreads();
-  if (threadIdx.x < (a.ts_target != nullptr ? 5 : 4)) atomicAdd(a.losses + threadIdx.x, (red[threadIdx.x][0] + red[threadIdx.x][1]) + (red[threadIdx.x][2] + red[threadIdx.x][3]));
 #pragma unroll
   for (int i = 0; i < 32; ++i) {
     if (i < a.n_act) {
       float s = warp_sum(gstd[i]);
-      if (lane == 0) atomicAdd(&sred[i], s);
+      if (lane == 0) red[5 + i][w] = s;
     }
   }
   __syncthreads();
-  if (threadIdx.x < a.n_act) atomicAdd(a.grad_std + threadIdx.x, sred[threadIdx.x]);
+  const int nq = 5 + a.n_act, q = threadIdx.x;
+  if (q < nq) a.part[(int64_t)blockIdx.x * LOSS_PART + q] = (red[q][0] + red[q][1]) + (red[q][2] + red[q][3]);
+  if (!last_block(a.ticket) || q >= nq) return;
+  float s = 0.0f;
+  for (int b = 0; b < (int)gridDim.x; ++b) s += __ldcg(a.part + (int64_t)b * LOSS_PART + q);
+  if (q >= 5) a.grad_std[q - 5] += s;
+  else if (q < 4 || a.ts_target != nullptr) a.losses[q] += s;
 }
 
 // DAgger loss PPO:273-276: mean_rows || sg(zp) - zh ||_2 ; writes d/d zh_pre (the derivative of the activation `act` folded in)
 __global__ void __launch_bounds__(128) dagger_loss_kernel(const float* __restrict__ zp, const float* __restrict__ zh, int zld, int latent,
-                                                          float* __restrict__ g, float* __restrict__ loss, int rows, int act) {
+                                                          float* __restrict__ g, float* __restrict__ loss, float* part, unsigned* ticket, int rows,
+                                                          int act) {
   __shared__ float red[4];
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   float l = 0.0f;
@@ -675,7 +708,11 @@ __global__ void __launch_bounds__(128) dagger_loss_kernel(const float* __restric
   float s = warp_sum(l);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
   __syncthreads();
-  if (threadIdx.x == 0) atomicAdd(loss, (red[0] + red[1]) + (red[2] + red[3]));
+  if (threadIdx.x == 0) part[blockIdx.x] = (red[0] + red[1]) + (red[2] + red[3]);      // this block's slot; the last block sums in order
+  if (!last_block(ticket) || threadIdx.x != 0) return;
+  float t = 0.0f;
+  for (int b = 0; b < (int)gridDim.x; ++b) t += __ldcg(part + b);
+  *loss += t;
 }
 
 // ---- backward -----------------------------------------------------------------------------------
@@ -830,7 +867,7 @@ static bool plan_chains(C2Chains& c, int what, const DwbcNetCfg& n, const float*
 }
 
 // every layer's weight gradient of both networks in one persistent launch (wgrad_group.cuh)
-static int weight_gradients(const DwbcNetCfg& n, float* grad, const DwbcStorage* s, const int64_t* idx, int rows, const Plan& p, cudaStream_t st) {
+static bool wgrad_gemms(WGroupBuilder& wb, const DwbcNetCfg& n, float* grad, const DwbcStorage* s, const int64_t* idx, const Plan& p) {
   const int Lld = (int)align_up(p.latent, 4);
   const BwdDescs d = bwd_descs(n, p);
   const int cnb = n.n_critic_layers, ctd = n.critic_dims[cnb - 1];
@@ -838,7 +875,6 @@ static int weight_gradients(const DwbcNetCfg& n, float* grad, const DwbcStorage*
   const int in0 = n.num_prop + p.latent, np = n.n_priv_layers;
   float* z = p.priv[np - 1];
   RowMat obs_all = rowmat_gather(s->observations, idx, s->obs_stride);
-  WGroupBuilder wb;
   head_wgrad(wb, grad, d.cl, act_mat(p.cb[cnb - 1], ctd), ctd);
   head_wgrad(wb, grad, d.ca, act_mat(p.cb[cnb - 1], ctd), ctd);
   for (int l = cnb - 1; l >= 0; --l) {
@@ -859,7 +895,11 @@ static int weight_gradients(const DwbcNetCfg& n, float* grad, const DwbcStorage*
     RowMat X = l == 0 ? rowmat_gather(s->observations + n.num_prop, idx, s->obs_stride) : rowmat(p.priv[l - 1], (int)align_up(in, 4));
     wb.add(rowmat(p.dzp[l], (int)align_up(n.priv_dims[l], 4)), X, grad + n.off_priv_w[l], in, grad + n.off_priv_b[l], n.priv_dims[l], in);
   }
-  if (!wb.ok) return DWBC_ERR_UNSUPPORTED;
+  return wb.ok;
+}
+static int weight_gradients(const DwbcNetCfg& n, float* grad, const DwbcStorage* s, const int64_t* idx, int rows, const Plan& p, cudaStream_t st) {
+  WGroupBuilder wb;
+  if (!wgrad_gemms(wb, n, grad, s, idx, p)) return DWBC_ERR_UNSUPPORTED;
   return launch_wgrad_group(wb.g, rows, mlp_precision == 2, st);
 }
 
@@ -969,7 +1009,7 @@ extern "C" int dwbc_ppo_minibatch_grad(const DwbcNetCfg* net, const float* param
     f.adv = s->advantages;
     f.zh = s->hist_latent ? s->hist_latent : p.zh; f.zh_ld = s->hist_latent ? s->hist_latent_ld : Lld; f.zh_by_src = s->hist_latent ? 1 : 0;
     f.g_leg = p.g_leg; f.gleg_ld = gleg_ld; f.g_arm = p.g_arm; f.garm_ld = garm_ld; f.g_v = p.g_vl; f.gv_ld = 4; f.g_z = p.g_z; f.gz_ld = Lld;
-    f.grad_std = grad + n.off_std; f.losses = losses_out;
+    f.grad_std = grad + n.off_std; f.losses = losses_out; f.part = p.loss_part;
     f.n_leg = n.n_leg; f.n_act = n.n_leg + n.n_arm; f.latent = p.latent; f.rows = rows;
     f.clip = hp->clip_param; f.c_value = hp->value_loss_coef; f.c_ent = hp->entropy_coef; f.c_reg = hp->priv_reg_coef; f.rho = hp->mixing_ratio;
     f.clipped_value = hp->use_clipped_value_loss;
@@ -988,7 +1028,7 @@ extern "C" int dwbc_ppo_minibatch_grad(const DwbcNetCfg* net, const float* param
   a.mean = p.mean; a.mean_ld = p.mean_ld; a.std = P + n.off_std; a.value = p.value; a.zp = z; a.zld = Lld; a.zh = s->hist_latent ? s->hist_latent : p.zh; a.zh_ld = s->hist_latent ? s->hist_latent_ld : Lld; a.zh_by_src = s->hist_latent ? 1 : 0;
   a.actions = s->actions; a.old_logp = s->log_prob; a.old_values = s->values; a.returns = s->returns; a.adv = s->advantages; a.idx = idx;
   a.g_leg = p.g_leg; a.gleg_ld = gleg_ld; a.g_arm = p.g_arm; a.garm_ld = garm_ld; a.g_vl = p.g_vl; a.g_va = p.g_va; a.gv_ld = 4; a.g_z = p.g_z;
-  a.grad_std = grad + n.off_std; a.losses = losses_out;
+  a.grad_std = grad + n.off_std; a.losses = losses_out; a.part = p.loss_part; a.ticket = reinterpret_cast<unsigned*>(p.queue + 2);
   a.rows = rows; a.n_leg = n.n_leg; a.n_act = n.n_leg + n.n_arm; a.latent = p.latent;
   a.clip = hp->clip_param; a.c_value = hp->value_loss_coef; a.c_ent = hp->entropy_coef; a.c_reg = hp->priv_reg_coef; a.rho = hp->mixing_ratio;
   a.clipped_value = hp->use_clipped_value_loss;
@@ -1080,7 +1120,8 @@ extern "C" int dwbc_dagger_minibatch_grad(const DwbcNetCfg* net, const float* pa
   if (cudaMemsetAsync(p.dhwl, 0, sizeof(float) * (32 * 36), st) != cudaSuccess) return DWBC_ERR_LAUNCH;
   TRY(priv_forward(n, P, s->observations, idx, s->obs_stride, rows, p, st));             // PPO:273-274 (no grad)
   TRY(hist_forward(n, P, s->observations, idx, s->obs_stride, rows, p, st));             // PPO:275
-  dagger_loss_kernel<<<(rows + 127) / 128, 128, 0, st>>>(p.priv[n.n_priv_layers - 1], p.zh, Lld, L, p.dzh, losses_out, rows, mlp_act);
+  dagger_loss_kernel<<<(rows + 127) / 128, 128, 0, st>>>(p.priv[n.n_priv_layers - 1], p.zh, Lld, L, p.dzh, losses_out, p.loss_part,
+                                                           reinterpret_cast<unsigned*>(p.queue + 3), rows, mlp_act);
   DWBC_LAUNCH_CHECK();
   // linear_output: zh = act(flat . Wl'^T + b)
   const float* hlast = p.hc[g.nconv - 1];
@@ -1113,6 +1154,19 @@ extern "C" int dwbc_dagger_minibatch_grad(const DwbcNetCfg* net, const float* pa
   return DWBC_OK;
 }
 
+// The weight-gradient partials of a debug entry point: `cap` floats of stream-ordered memory, freed behind the launches
+template <class F>
+static int with_debug_wpart(int64_t cap, cudaStream_t st, F&& launch) {
+  void* p = nullptr;
+  if (cudaMallocAsync(&p, (size_t)cap * sizeof(float), st) != cudaSuccess) return DWBC_ERR_LAUNCH;
+  mlp_wpart = static_cast<float*>(p);
+  mlp_wpart_cap = cap;
+  const int rc = launch();
+  mlp_wpart = nullptr;
+  mlp_wpart_cap = 0;
+  return cudaFreeAsync(p, st) == cudaSuccess ? rc : DWBC_ERR_LAUNCH;
+}
+
 // Debug / test entry: one GEMM of the selected implementation on plain row-major device matrices.
 //   mode 0: Y[M,N] = act(X[M,K] W[N,K]^T + b)      mode 1: dX[M,N] = G[M,K] W[K,N]      mode 2: dW[M,N] += G[K,M]^T X[K,N], db += colsum(G)
 extern "C" int dwbc_debug_gemm(int mode, int tc, const float* A, int64_t lda, const float* Bm, int64_t ldb, float* C, int64_t ldc,
@@ -1123,7 +1177,12 @@ extern "C" int dwbc_debug_gemm(int mode, int tc, const float* A, int64_t lda, co
   cudaStream_t st = (cudaStream_t)stream;
   if (mode == 0) rc = linear_fwd(rowmat(A, lda), Bm, ldb, bias, C, ldc, M, N, K, act, 0, st);
   else if (mode == 1) rc = linear_bwd_data(rowmat(A, lda), Bm, ldb, C, ldc, M, N, K, ACT_NONE, RowMat{}, 0, st);
-  else rc = linear_bwd_weight(rowmat(A, lda), rowmat(Bm, ldb), C, ldc, dbias, K, M, N, st);
+  else {
+    // the partials of the split-K / slab sums in stream-ordered scratch (no workspace here)
+    if (M <= 0 || N <= 0 || K <= 0) { mlp_precision = saved; return DWBC_ERR_ARG; }
+    const int64_t cap = std::max(simt_wgrad_floats(M, N, K), wg_max_nslab(K) * wg_slot(std::min(M, 128), std::min(N, 128)));
+    rc = with_debug_wpart(cap, st, [&] { return linear_bwd_weight(rowmat(A, lda), rowmat(Bm, ldb), C, ldc, dbias, K, M, N, st); });
+  }
   mlp_precision = saved;
   return rc;
 }
@@ -1202,7 +1261,10 @@ extern "C" int dwbc_debug_wgrad_group(const DwbcWgradGemm* gemms, int n, int row
     b.add(mat(d.g, d.g_idx, (int)d.g_image, d.g_ld), mat(d.x, d.x_idx, (int)d.x_image, d.x_ld), d.dw, d.lddw, d.db, (int)d.mo, (int)d.ni);
   }
   if (!b.ok) return DWBC_ERR_ARG;
-  return launch_wgrad_group(b.g, rows, x3 != 0, reinterpret_cast<cudaStream_t>(stream));
+  int64_t slots = 0;
+  for (int i = 0; i < n; ++i) slots += wg_slot((int)gemms[i].mo, (int)gemms[i].ni);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  return with_debug_wpart(wg_max_nslab(rows) * slots, st, [&] { return launch_wgrad_group(b.g, rows, x3 != 0, st); });
 }
 extern "C" int dwbc_debug_set_wgrad_items(int per_cta) {
   if (per_cta < 1 || per_cta > 64) return DWBC_ERR_ARG;
@@ -1216,4 +1278,23 @@ extern "C" int dwbc_debug_set_chain_singles(int n) {
 }
 extern "C" int dwbc_debug_set_tc_cycle_buffer(unsigned long long* dev_ptr) {
   return cudaMemcpyToSymbol(g_tc_cycles, &dev_ptr, sizeof(dev_ptr)) == cudaSuccess ? DWBC_OK : DWBC_ERR_LAUNCH;
+}
+
+// The partial area the grouped weight-gradient launch of dwbc_ppo_minibatch_grad would use on `sms` SMs with `items` per CTA, and the
+// area dwbc_workspace_bytes reserves for it (host code only, no GPU; tests/test_reproducibility_cpu.py checks need <= bound)
+extern "C" int dwbc_debug_wgrad_partials(const DwbcNetCfg* net, int32_t rows, int sms, int items, int64_t* need, int64_t* bound) {
+  TRY(check_net(net));
+  if (rows <= 0 || sms <= 0 || items < 1 || items > 64 || !need || !bound) return DWBC_ERR_ARG;
+  float* const ws = reinterpret_cast<float*>(uintptr_t(1) << 40);
+  DwbcStorage s{};
+  s.observations = reinterpret_cast<const float*>(uintptr_t(2) << 40);
+  s.obs_stride = net->num_obs;
+  Plan p = make_plan(*net, rows, ws);
+  mlp_wpart = nullptr;
+  mlp_wpart_cap = 0;
+  WGroupBuilder wb;
+  if (!wgrad_gemms(wb, *net, ws, &s, reinterpret_cast<const int64_t*>(uintptr_t(3) << 40), p)) return DWBC_ERR_UNSUPPORTED;
+  *need = wg_plan(wb.g, rows, mlp_precision == 2, sms, items);
+  *bound = wpart_floats(*net, rows);
+  return DWBC_OK;
 }

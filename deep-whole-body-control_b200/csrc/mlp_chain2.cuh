@@ -90,6 +90,7 @@ struct FinArgs {
   const float* zh; int64_t zh_ld; int zh_by_src;
   float* g_leg; int gleg_ld; float* g_arm; int garm_ld; float* g_v; int gv_ld; float* g_z; int gz_ld;
   float* grad_std; float* losses;
+  float* part;                                               // [rows / 16][C2_FIN_PART] partial sums, one slot per (tile, worker warp)
   int n_leg, n_act, latent, rows;
   float clip, c_value, c_ent, c_reg, rho;
   int clipped_value;
@@ -154,8 +155,14 @@ __global__ void pack_weights2_kernel(const __grid_constant__ C2PackList pl) {
 // ---- device helpers ---------------------------------------------------------------------------------------------------
 struct C2Shared {
   uint64_t w_full, w_free, ld_bar;
-  int item;
+  int item, last;
 };
+
+// Slot of the update hooks' warp sums: a worker warp owns 16 rows of a tile, so row m belongs to slot m / 16 = 8 tile + warp.  The last
+// CTA adds the slots up in slot order (c2_fin_reduce): the sums do not depend on which CTA ran which tile.
+constexpr int C2_FIN_PART = 40;
+enum { C2P_STD = 0, C2P_SURR = 32, C2P_ENT = 34, C2P_VAL = 36, C2P_REG = 38, C2P_TS = 39 };   // (SURR, ENT, VAL: one per channel)
+__device__ __forceinline__ float* c2_fin_slot(const FinArgs& f, int64_t m) { return f.part + (m >> 4) * C2_FIN_PART; }
 
 __device__ __forceinline__ void c2_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(tc_smem_u32(bar)), "r"(bytes) : "memory");
@@ -370,8 +377,9 @@ __device__ __forceinline__ void c2_fin_ppo(const FinArgs& f, int c, int64_t m, b
         if (i < gld) grow[i] = gm[i];
     }
   }
+  float* slot = c2_fin_slot(f, m);
 #pragma unroll
-  for (int i = 0; i < C2_GRP; ++i) {           // gradient of std: one atomic per warp and column
+  for (int i = 0; i < C2_GRP; ++i) {           // gradient of std: one warp sum per column
     if (i < cnt) {                             // (warp-uniform)
       float gs = 0.0f;
       if (on) {
@@ -379,14 +387,14 @@ __device__ __forceinline__ void c2_fin_ppo(const FinArgs& f, int c, int64_t m, b
         gs = glp * ((d * d) / (sg[i] * sg[i] * sg[i]) - 1.0f / sg[i]) - f.c_ent * inv2m / sg[i];
       }
       gs = warp_sum(gs);
-      if (lane == 0) atomicAdd(f.grad_std + off + i, gs);
+      if (lane == 0) slot[C2P_STD + off + i] = gs;
     }
   }
   const float ss = warp_sum(l_surr * inv2m), se = warp_sum(l_ent * inv2m);
-  if (lane == 0) { atomicAdd(f.losses + 0, ss); atomicAdd(f.losses + 1 + 2, se); }
+  if (lane == 0) { slot[C2P_SURR + c] = ss; slot[C2P_ENT + c] = se; }
   if (c == 1 && f.ts_target != nullptr) {          // (warp-uniform)
     const float st = warp_sum(l_ts / ((float)f.rows * (float)cnt));
-    if (lane == 0) atomicAdd(f.losses + 4, st);
+    if (lane == 0) slot[C2P_TS] = st;
   }
 }
 // FIN_VALUE (PPO:209-216), channel c
@@ -414,7 +422,7 @@ __device__ __forceinline__ void c2_fin_value(const FinArgs& f, int c, int64_t m,
     if (c == 0) for (int i = 2; i < f.gv_ld; ++i) f.g_v[m * f.gv_ld + i] = 0.0f;     // pad columns are operand columns of the backward pass
   }
   const float s = warp_sum(l_val * inv2m);
-  if (lane == 0) atomicAdd(f.losses + 1, s);
+  if (lane == 0) c2_fin_slot(f, m)[C2P_VAL + c] = s;
 }
 // FIN_REG (PPO:174-177): || z_priv - sg(z_hist) ||_2 per row, mean over rows
 __device__ __forceinline__ void c2_fin_reg(const FinArgs& f, int64_t m, bool on, const float* v, int lane) {
@@ -433,7 +441,38 @@ __device__ __forceinline__ void c2_fin_reg(const FinArgs& f, int64_t m, bool on,
       if (i < f.gz_ld) f.g_z[m * f.gz_ld + i] = i < f.latent ? s * (v[i] - zhr[i]) : 0.0f;
   }
   const float s = warp_sum(nrm * invm);
-  if (lane == 0) atomicAdd(f.losses + 2, s);
+  if (lane == 0) c2_fin_slot(f, m)[C2P_REG] = s;
+}
+// The last CTA of an update's forward launch: the slots of all (tile, warp) pairs in slot order, into the std gradient and the loss
+// means.  Worker thread q + 40 p sums field q over the p-th of six contiguous slot ranges; the six range sums are then added in order.
+// Fields no hook of this launch wrote (std columns >= n_act, C2P_TS without torque supervision) may hold what a call with more rows left
+// in a shared workspace: they are summed like the others but never used.
+__device__ __forceinline__ void c2_fin_reduce(const FinArgs& f, int tiles, float* scratch, int tid) {
+  constexpr int NPART = 6;
+  const int nslot = tiles * C2_WORKERS, q = tid % C2_FIN_PART, p = tid / C2_FIN_PART;
+  if (p < NPART) {
+    const int b = (int)((int64_t)nslot * p / NPART), e = (int)((int64_t)nslot * (p + 1) / NPART);
+    float s = 0.0f;
+#pragma unroll 8
+    for (int k = b; k < e; ++k) s += __ldcg(f.part + (int64_t)k * C2_FIN_PART + q);
+    scratch[p * C2_FIN_PART + q] = s;
+  }
+  c2_wbar();
+  if (tid < C2_FIN_PART) {
+    float t = 0.0f;
+    for (int i = 0; i < NPART; ++i) t += scratch[i * C2_FIN_PART + tid];
+    scratch[NPART * C2_FIN_PART + tid] = t;
+  }
+  c2_wbar();
+  const float* tot = scratch + NPART * C2_FIN_PART;
+  if (tid < f.n_act) f.grad_std[tid] += tot[C2P_STD + tid];
+  if (tid == 0) {
+    f.losses[0] += tot[C2P_SURR] + tot[C2P_SURR + 1];
+    f.losses[1] += tot[C2P_VAL] + tot[C2P_VAL + 1];
+    f.losses[2] += tot[C2P_REG];
+    f.losses[3] += tot[C2P_ENT] + tot[C2P_ENT + 1];
+    if (f.ts_target != nullptr) f.losses[4] += tot[C2P_TS];
+  }
 }
 
 // ---- the kernel -------------------------------------------------------------------------------------------------------
@@ -795,11 +834,15 @@ __global__ void __launch_bounds__(C2_THREADS, 1) chain2_kernel(const __grid_cons
     }
   }
   if (tid == 0) c2_bulk_wait_all();      // the image stores of this CTA have landed
+  __threadfence();                       // (and the partial sums of the update hooks)
   __syncthreads();
   if (tid == 0) {                        // the last CTA re-arms the queue for the next launch
     __threadfence();
-    if (atomicAdd(L.queue + 1, 1) == (int)gridDim.x - 1) { L.queue[0] = 0; L.queue[1] = 0; __threadfence(); }
+    sh.last = atomicAdd(L.queue + 1, 1) == (int)gridDim.x - 1;
+    if (sh.last) { L.queue[0] = 0; L.queue[1] = 0; __threadfence(); }
   }
+  __syncthreads();
+  if (sh.last && L.fin.losses != nullptr && warp < C2_WORKERS) c2_fin_reduce(L.fin, tiles, c2_smem, tid);
 }
 
 

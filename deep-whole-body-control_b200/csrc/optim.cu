@@ -6,6 +6,8 @@
 
 namespace dwbc {
 
+// Per-block partial sums of squares: block b writes out[b].  clip_adam_kernel adds them up in block order, so the norm does not depend on
+// which block finished first.
 __global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ g, int64_t n, float scale, double* __restrict__ out) {
   __shared__ double red[8];
   double s = 0.0;
@@ -19,7 +21,7 @@ __global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ g,
   if (threadIdx.x == 0) {
     double t = 0.0;
     for (int i = 0; i < 8; ++i) t += red[i];
-    atomicAdd(out, t);
+    out[blockIdx.x] = t;
   }
 }
 
@@ -27,12 +29,28 @@ struct AdamArgs {
   float* p; float* g; float* m; float* v;
   int64_t n;
   float scale, max_norm, beta1, beta2, eps, step_size, bc2_sqrt;
-  const double* sumsq;
+  const double* sumsq;                   // [nparts] partials of sumsq_kernel
+  int nparts;
   float* norm_out;
 };
 
+// Every block sums the partials itself, in the same fixed order (thread t: partials t, t + 256, ...; then a fixed tree)
+__device__ __forceinline__ double sum_partials(const double* __restrict__ part, int n) {
+  __shared__ double red[256];
+  double s = 0.0;
+  for (int i = threadIdx.x; i < n; i += 256) s += part[i];
+  red[threadIdx.x] = s;
+  __syncthreads();
+#pragma unroll
+  for (int w = 128; w > 0; w >>= 1) {
+    if ((int)threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+    __syncthreads();
+  }
+  return red[0];
+}
+
 __global__ void __launch_bounds__(256) clip_adam_kernel(const AdamArgs a) {
-  const float total = (float)sqrt(*a.sumsq);                        // clip_grad_norm_: ||g||_2 over all tensors
+  const float total = (float)sqrt(sum_partials(a.sumsq, a.nparts));  // clip_grad_norm_: ||g||_2 over all tensors
   const float coef = fminf(a.max_norm / (total + 1e-6f), 1.0f);
   if (a.norm_out && blockIdx.x == 0 && threadIdx.x == 0) *a.norm_out = total;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += (int64_t)gridDim.x * blockDim.x) {
@@ -61,16 +79,15 @@ extern "C" int dwbc_clip_adam_step(float* params, float* grad, float* adam_m, fl
                                    dwbc_stream_t stream) {
   if (!params || !grad || !adam_m || !adam_v || !hp || !norm_scratch || count <= 0 || first < 0 || step < 1) return DWBC_ERR_ARG;
   cudaStream_t st = (cudaStream_t)stream;
-  if (cudaMemsetAsync(norm_scratch, 0, sizeof(double), st) != cudaSuccess) return DWBC_ERR_LAUNCH;
   const float scale = hp->grad_scale == 0.0f ? 1.0f : hp->grad_scale;
   int grid = (int)((count + 1023) / 1024);
-  if (grid > 592) grid = 592;
+  if (grid > DWBC_NORM_SCRATCH) grid = DWBC_NORM_SCRATCH;
   if (grid < 1) grid = 1;
   sumsq_kernel<<<grid, 256, 0, st>>>(grad + first, count, scale, norm_scratch);
   DWBC_LAUNCH_CHECK();
   const double bc1 = 1.0 - pow((double)hp->beta1, (double)step), bc2 = 1.0 - pow((double)hp->beta2, (double)step);
   AdamArgs a{params + first, grad + first, adam_m + first, adam_v + first, count, scale, hp->max_grad_norm, hp->beta1, hp->beta2,
-             hp->adam_eps, (float)((double)hp->lr / bc1), (float)sqrt(bc2), norm_scratch, grad_norm_out};
+             hp->adam_eps, (float)((double)hp->lr / bc1), (float)sqrt(bc2), norm_scratch, grid, grad_norm_out};
   clip_adam_kernel<<<grid, 256, 0, st>>>(a);
   DWBC_LAUNCH_CHECK();
   return DWBC_OK;

@@ -8,7 +8,8 @@
 // The contraction index is the ROW of both sources, and wgmma takes TF32 operands K-major only.  Chunks of 32 rows are staged in their
 // source layout with 16-byte cp.async several chunks ahead; one pass per chunk writes them as K-major tiles (with the zero fill, the
 // 3xTF32 low parts and the bias sums), then the two warpgroups, owning output rows [0, 64) and [64, 128), multiply.  Each keeps its
-// accumulator in registers over the whole slab and reduces it into dW with vector atomics at the end.
+// accumulator in registers over the whole slab and stores it, with the slab's bias sums, to the slab's slot of the partial area; a
+// second pass (partials_reduce_kernel) adds the slots of each GEMM up in slab order into dW and db, so the sums repeat bit for bit.
 #pragma once
 #include <stdlib.h>
 
@@ -34,12 +35,14 @@ struct WGItem {
   float* db;            // nullable
   int Mo, Ni;
   int nslab, first;     // work items of this GEMM, index of its first item (set by launch_wgrad_group)
+  int64_t part;         // slot of slab 0 in the partial area; slab s at part + s * wg_slot(Mo, Ni): [Mo x Ni] dW, then [Mo] db
 };
+inline __host__ __device__ int64_t wg_slot(int Mo, int Ni) { return ((int64_t)Mo * Ni + Mo + 3) & ~(int64_t)3; }
 // Work items are enumerated GEMM by GEMM, GEMMs in the order launch_wgrad_group sorted them (longest item first).
 // snake == 0: item e goes to CTA e % grid (round-robin); snake != 0: round j of the deal runs forwards for even j, backwards for odd j.
 // Slab s of a GEMM with n slabs covers rows [b(s), b(s + 1)), b(s) = floor(s rows / n) rounded down to a whole chunk, b(n) = rows.
 // rev != 0: the slabs of a GEMM are taken from the LAST rows to the first.
-struct WGroup { int n, rows, items, snake, rev; WGItem it[WG_MAX]; };
+struct WGroup { int n, rows, items, snake, rev; float* part; WGItem it[WG_MAX]; };
 
 __device__ __forceinline__ void wg_cp16(float* dst, const float* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(tc_smem_u32(dst)), "l"(src) : "memory");
@@ -119,10 +122,12 @@ __device__ __forceinline__ void wg_mma_chunk(float* acc, uint32_t a0, uint32_t b
   wg_commit();
 }
 
+__shared__ float wg_bhalf[2][128];                    // the two row halves of a slab's bias sums
+
 // rows [k_begin, k_end) of one GEMM, N = the instruction width that covers Ni.  Per chunk c: wait for its copies, transpose it, refill
 // its stage with chunk c + stages and multiply it; the copies of the next stages - 1 chunks are in flight all the while.
 template <int N, bool X3>
-__device__ __forceinline__ void wg_slab(const WGItem& g, int64_t k_begin, int64_t k_end, float* smem, int tid, int warp, int lane) {
+__device__ __forceinline__ void wg_slab(const WGItem& g, int64_t k_begin, int64_t k_end, float* slot, float* smem, int tid, int warp, int lane) {
   constexpr int NS = wg_stages<X3>();
   const int Mo = g.Mo, Ni = g.Ni, mw = Mo <= 64 ? 64 : 128, wgi = warp >> 2;
   const bool mma_on = 64 * wgi < Mo;
@@ -170,19 +175,22 @@ __device__ __forceinline__ void wg_slab(const WGItem& g, int64_t k_begin, int64_
       wg_wait<0>();
     }
   }
-  // bias gradient: lanes l, l + 8, l + 16, l + 24 hold feature l % 8 of a step; warps 2i and 2i + 1 the two row halves
+  // bias gradient: lanes l, l + 8, l + 16, l + 24 hold feature l % 8 of a step; warps 2i and 2i + 1 the two row halves, added in that order
   if (g.db != nullptr) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       float b = bsum[j];
       b += __shfl_xor_sync(0xffffffffu, b, 8);
       b += __shfl_xor_sync(0xffffffffu, b, 16);
-      const int f = 8 * ((warp + 8 * j) >> 1) + lane;
-      if (lane < 8 && warp + 8 * j < mw / 4 && f < Mo) atomicAdd(g.db + f, b);
+      const int u = warp + 8 * j, f = 8 * (u >> 1) + lane;
+      if (lane < 8 && u < mw / 4 && f < Mo) wg_bhalf[u & 1][f] = b;
     }
+    __syncthreads();
+    if (tid < Mo) slot[(int64_t)Mo * Ni + tid] = wg_bhalf[0][tid] + wg_bhalf[1][tid];
+    __syncthreads();                                  // (wg_bhalf is reused by the next slab)
   }
-  // split-K partial straight from the fragments: lane l holds rows l/4 and l/4 + 8 of its warp's 16, columns 8 jj + 2 (l%4) + {0, 1}
-  const bool v2 = (g.lddw & 1) == 0 && (reinterpret_cast<uintptr_t>(g.dW) & 7) == 0;
+  // the slab's partial straight from the fragments: lane l holds rows l/4 and l/4 + 8 of its warp's 16, columns 8 jj + 2 (l%4) + {0, 1}
+  const bool v2 = (Ni & 1) == 0;                      // (slots start 16-byte aligned)
   if (mma_on) {
 #pragma unroll
     for (int jj = 0; jj < N / 8; ++jj) {
@@ -192,10 +200,10 @@ __device__ __forceinline__ void wg_slab(const WGItem& g, int64_t k_begin, int64_
       for (int e = 0; e < 2; ++e) {
         const int row = 64 * wgi + 16 * (warp & 3) + (lane >> 2) + 8 * e;
         if (row >= Mo) continue;
-        float* dst = g.dW + (int64_t)row * g.lddw + col;
+        float* dst = slot + (int64_t)row * Ni + col;
         const float x0 = acc[4 * jj + 2 * e], x1 = acc[4 * jj + 2 * e + 1];
-        if (v2 && col + 1 < Ni) asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(x0), "f"(x1) : "memory");
-        else { atomicAdd(dst, x0); if (col + 1 < Ni) atomicAdd(dst + 1, x1); }
+        if (v2) *reinterpret_cast<float2*>(dst) = make_float2(x0, x1);
+        else { dst[0] = x0; if (col + 1 < Ni) dst[1] = x1; }
       }
     }
   }
@@ -221,10 +229,11 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_group_kernel(const __grid
     const int64_t k_begin = (int64_t)slab_i * grp.rows / g.nslab / WG_KC * WG_KC;
     const int64_t k_end = slab_i + 1 == g.nslab ? (int64_t)grp.rows : (int64_t)(slab_i + 1) * grp.rows / g.nslab / WG_KC * WG_KC;
     if (k_end <= k_begin) continue;
+    float* slot = grp.part + g.part + (int64_t)slab_i * wg_slot(g.Mo, g.Ni);
     const int nw = wg_width((g.Ni + 15) & ~15);
-    if (nw == 32) wg_slab<32, X3>(g, k_begin, k_end, wg_smem, tid, warp, lane);
-    else if (nw == 64) wg_slab<64, X3>(g, k_begin, k_end, wg_smem, tid, warp, lane);
-    else wg_slab<128, X3>(g, k_begin, k_end, wg_smem, tid, warp, lane);
+    if (nw == 32) wg_slab<32, X3>(g, k_begin, k_end, slot, wg_smem, tid, warp, lane);
+    else if (nw == 64) wg_slab<64, X3>(g, k_begin, k_end, slot, wg_smem, tid, warp, lane);
+    else wg_slab<128, X3>(g, k_begin, k_end, slot, wg_smem, tid, warp, lane);
   }
 }
 
@@ -240,6 +249,13 @@ struct WGroupBuilder {
 
 // Longest slab: the accumulator sums a slab's rows in registers, and longer sums lose accuracy against the fp32 reference
 constexpr int64_t WG_MAX_SLAB = 1024;
+// Most slabs of one GEMM: the fewer of one per four chunks and WG_MAX_NSLAB, unless rows / WG_MAX_SLAB needs more.  It bounds the
+// partial area by wg_max_nslab(rows) x the GEMMs' slots, whatever the SM count and the items per CTA (dwbc_workspace_bytes).
+constexpr int64_t WG_MAX_NSLAB = 128;
+inline int64_t wg_max_nslab(int64_t rows) {
+  const int64_t lo = (rows + WG_MAX_SLAB - WG_KC - 1) / (WG_MAX_SLAB - WG_KC);
+  return std::max<int64_t>(1, std::min(rows / (4 * WG_KC), std::max(lo, WG_MAX_NSLAB)));
+}
 inline int wg_items_per_cta = 4;                     // tuning aid (dwbc_debug_set_wgrad_items)
 inline int wg_reverse = 0;                            // tuning aid (dwbc_debug_set_wgrad_reverse): 0 = slabs from the first rows upwards
 inline int wg_snake = 0;                             // tuning aid (dwbc_debug_set_wgrad_snake): 0 = round-robin deal
@@ -259,16 +275,8 @@ inline double wg_row_cost(const WGItem& it, bool x3) {
 // at least rows / WG_MAX_SLAB, at most one per four chunks), so its slabs are the shorter the more a row costs.  The GEMMs are then ordered
 // by the cost of one of their items, longest first, so that items rounded short fill the end of the launch.  At small row counts the
 // limits leave fewer items.
-inline int launch_wgrad_group(WGroup& g, int rows, bool x3, cudaStream_t st) {
-  if (g.n <= 0 || rows <= 0) return DWBC_ERR_ARG;
-  g.snake = wg_snake;
-  g.rev = wg_reverse;
-  static int sms = 0;
-  if (!sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  }
+// The plan on `sms` SMs with `items_per_cta` (host code); returns the floats of partial area it needs.
+inline int64_t wg_plan(WGroup& g, int rows, bool x3, int sms, int items_per_cta) {
   g.rows = rows;
   double cost[WG_MAX], total = 0.0, cmin = 1e30;
   for (int i = 0; i < g.n; ++i) {
@@ -276,9 +284,9 @@ inline int launch_wgrad_group(WGroup& g, int rows, bool x3, cudaStream_t st) {
     cmin = std::min(cmin, cost[i]);
   }
   const int64_t span = WG_MAX_SLAB - WG_KC;           // rows / n, before the slab bounds are rounded down to whole chunks
-  const int64_t per_cta = std::max<int64_t>(wg_items_per_cta, (int64_t)std::ceil((double)rows * total / ((double)sms * span * cmin) - 1e-9));
+  const int64_t per_cta = std::max<int64_t>(items_per_cta, (int64_t)std::ceil((double)rows * total / ((double)sms * span * cmin) - 1e-9));
   const int64_t target = per_cta * sms;
-  const int64_t lo = (rows + span - 1) / span, hi = std::max<int64_t>(1, rows / (4 * WG_KC));
+  const int64_t lo = (rows + span - 1) / span, hi = wg_max_nslab(rows);
   int64_t n[WG_MAX], sum = 0;
   double share[WG_MAX];
   for (int i = 0; i < g.n; ++i) {
@@ -310,6 +318,28 @@ inline int launch_wgrad_group(WGroup& g, int rows, bool x3, cudaStream_t st) {
   }
   std::copy(sorted, sorted + g.n, g.it);
   g.items = items;
+  int64_t need = 0;
+  for (int i = 0; i < g.n; ++i) {
+    g.it[i].part = need;
+    need += (int64_t)g.it[i].nslab * wg_slot(g.it[i].Mo, g.it[i].Ni);
+  }
+  return need;
+}
+
+inline int launch_wgrad_group(WGroup& g, int rows, bool x3, cudaStream_t st) {
+  if (g.n <= 0 || rows <= 0) return DWBC_ERR_ARG;
+  g.snake = wg_snake;
+  g.rev = wg_reverse;
+  static int sms = 0;
+  if (!sms) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  }
+  const int64_t need = wg_plan(g, rows, x3, sms, wg_items_per_cta);
+  const int items = g.items;
+  g.part = mlp_wpart;
+  if (!g.part || need > mlp_wpart_cap || (reinterpret_cast<uintptr_t>(g.part) & 15)) return DWBC_ERR_ARG;
   const int grid = items < sms ? items : sms;
   static bool attr = false;
   if (!attr) {
@@ -321,7 +351,15 @@ inline int launch_wgrad_group(WGroup& g, int rows, bool x3, cudaStream_t st) {
   if (x3) wgrad_group_kernel<true><<<grid, WG_THREADS, WG_SMEM, st>>>(g);
   else wgrad_group_kernel<false><<<grid, WG_THREADS, WG_SMEM, st>>>(g);
   ++dwbc_launch_counter;
-  return cudaGetLastError() == cudaSuccess ? DWBC_OK : DWBC_ERR_LAUNCH;
+  if (cudaGetLastError() != cudaSuccess) return DWBC_ERR_LAUNCH;
+  RedBuilder r;                                        // every GEMM's slabs in slab order
+  for (int i = 0; i < g.n; ++i) {
+    const WGItem& it = g.it[i];
+    const int64_t s = wg_slot(it.Mo, it.Ni);
+    r.add(it.dW, it.lddw, it.Mo, it.Ni, it.part, s, it.nslab);
+    if (it.db) r.add(it.db, 0, 1, it.Mo, it.part + (int64_t)it.Mo * it.Ni, s, it.nslab);
+  }
+  return r.launch(g.part, st);
 }
 
 // one weight gradient on its own (the layer-wise path): dW[M x N] += A^T B over K rows, db += colsum(A)

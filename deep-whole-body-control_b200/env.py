@@ -140,6 +140,7 @@ class FusedWidowGo1Core:
         self.episode_sums = {k: self._sums[:, i] for i, k in enumerate(self.sum_names)}
         self.episode_metric_sums = {k: self._sums[:, len(self.sum_names) + i] for i, k in enumerate(METRIC_NAMES)}
         self._stats = z(1 + self._sums_stride)
+        self._stats_scratch = z(N, self._sums_stride)    # per-env slots of the ended episodes' sums (episode_scratch)
         self._pd = None
         # --- terrain ---
         self.height_samples = None
@@ -316,6 +317,7 @@ class FusedWidowGo1Core:
         b.obs_buf, b.obs_stride = self.obs_buf.data_ptr(), self.obs_buf.stride(0)
         b.rew_buf, b.arm_rew_buf = P(self.rew_buf), P(self.arm_rew_buf)
         b.reset_buf, b.time_out_buf, b.episode_stats = P(self.reset_buf), P(self.time_out_buf), P(self._stats)
+        b.episode_scratch = P(self._stats_scratch)
 
     # ------------------------------------------------------------------ curriculum (WG:678-692)
     def update_command_curriculum(self):

@@ -89,7 +89,7 @@ class FusedPPO:
         self.hist_encoder_optimizer = _AdamState(ac, hf, hc, learning_rate)               # PPO:79
         self.grad = torch.zeros_like(ac.flat)
         self._losses = torch.zeros(5, device=self.device)        # surrogate, value, priv_reg, entropy, arm torques
-        self._norm_scratch = torch.zeros(2, dtype=torch.float64, device=self.device)
+        self._norm_scratch = torch.zeros(L.NORM_SCRATCH, dtype=torch.float64, device=self.device)
         self._grad_norm = torch.zeros(1, device=self.device)
         self._ws = None
         self._ws_rows = 0

@@ -44,7 +44,7 @@ class FusedRolloutStorage:
         self.actions_log_prob, self.values = z(T, N, 2), z(T, N, 2)
         self.returns, self.advantages = z(T, N, 2), z(T, N, 2)
         self.mu, self.sigma = z(T, N, *actions_shape), z(T, N, *actions_shape)
-        self._stats = torch.zeros(3, dtype=torch.float64, device=self.device)
+        self._stats = torch.zeros(L.GAE_STATS, dtype=torch.float64, device=self.device)   # (n, sum, sum sq), then dwbc_gae's partials
         self.step = 0
         self._lib = L.lib()
         self._c = L.Storage()
@@ -86,7 +86,7 @@ class FusedRolloutStorage:
                                    L.ptr(self.returns), L.ptr(self.advantages), L.ptr(self._stats), T, N, gamma, lam, int(fused),
                                    L.stream_ptr()), "dwbc_gae")
         if not fused:
-            shard.allreduce_adv_stats_(self._stats, world_size, group)
+            shard.allreduce_adv_stats_(self._stats[:3], world_size, group)
             L.check(self._lib.dwbc_normalize_advantages(L.ptr(self.advantages), L.ptr(self._stats), T * N * 2, L.stream_ptr()),
                     "dwbc_normalize_advantages")
 

@@ -164,8 +164,10 @@ typedef struct DwbcEnvBuffers {
   float* arm_rew_buf;            /* [N] */
   uint8_t* reset_buf;            /* [N] torch.bool */
   uint8_t* time_out_buf;         /* [N] torch.bool */
-  float* episode_stats;          /* [1+sums_stride]: #resets, then per-slot sum over reset envs (atomics;
-                                    caller zeroes before the step; WG:743-750 means = sum/count/T_ep) */
+  float* episode_stats;          /* [1+sums_stride]: += #resets, then += per-slot sum over the envs that reset this step, added in
+                                    env order (bitwise repeatable); the caller zeroes it when it starts a new count
+                                    (WG:743-750 means = sum/count/T_ep) */
+  float* episode_scratch;        /* [N,sums_stride] scratch: the ended episodes' sums of the envs that reset (no initialisation) */
   /* optional direct-to-storage transition (SURVEY 8f row f2): with store_rewards != NULL the kernel also performs
    * PPO.process_env_step's reward path (PPO:130-134) and the dones store (RS:102) of this step:
    *   store_rewards[n,:] = (rew, arm_rew) + store_gamma * store_values[n,:] * time_out[n];  store_dones[n] = reset[n]  */
@@ -223,9 +225,13 @@ int dwbc_store_rewards(const float* rew, const float* arm_rew, const float* valu
 /* RolloutStorage.compute_returns (RS:136-150): two-channel GAE backward scan over
  * rewards/values [T,N,2], dones [T,N] uint8, last_values [N,2] -> returns, advantages [T,N,2];
  * advantages are normalised jointly over all T*N*2 elements with the UNBIASED std + 1e-8.
- * stats[3] (double: n, sum, sum of squares) is device scratch the caller zeroes.  With
- * normalize == 0 the raw advantages are written and stats filled (multi-GPU: all-reduce stats,
- * then call dwbc_normalize_advantages). */
+ * stats[DWBC_GAE_STATS] (double) is device scratch the caller zeroes: stats[0..2] receive (n, sum,
+ * sum of squares) of the raw advantages; the rest holds one (sum, sum of squares) partial per block,
+ * added up in block order, and a counter that every call leaves at zero.  With normalize == 0 the
+ * raw advantages are written and stats[0..2] filled (multi-GPU: all-reduce stats[0..2], then call
+ * dwbc_normalize_advantages). */
+#define DWBC_GAE_MAX_BLOCKS 1024
+#define DWBC_GAE_STATS (4 + 2 * DWBC_GAE_MAX_BLOCKS)
 int dwbc_gae(const float* rewards, const float* values, const uint8_t* dones, const float* last_values, float* returns,
              float* advantages, double* stats, int32_t T, int32_t N, float gamma, float lam, int32_t normalize,
              dwbc_stream_t stream);
@@ -303,8 +309,10 @@ int dwbc_compute_torques(const DwbcPdCfg* cfg, const float* actions, const float
                          float* torques, int32_t num_envs, dwbc_stream_t stream);
 
 /* Bytes of device workspace the forward / update entry points need for `rows` rows.  The workspace must be ZERO-FILLED when it is
- * first handed to the library (its first 256 bytes hold the work-queue counters of the fused chain kernel, which every launch leaves
- * at zero again); one workspace sized for the largest `rows` may be shared by calls with smaller `rows`. */
+ * first handed to the library (its first 256 bytes hold counters -- the work queue of the fused chain kernel and the tickets of the
+ * fixed-order loss sums -- which every launch leaves at zero again); one workspace sized for the largest `rows` may be shared by calls
+ * with smaller `rows`.  The workspace also holds the partials of every cross-CTA sum (loss means, std gradient, weight gradients), which
+ * are added up in a fixed order: the results repeat bit for bit. */
 int64_t dwbc_workspace_bytes(const DwbcNetCfg* net, int64_t rows);
 
 /* PPO.act (PPO:115-127 = AC:337-353): obs[N,obs_stride] -> mean, sigma, actions = mean +
@@ -363,8 +371,11 @@ int dwbc_dagger_minibatch_grad(const DwbcNetCfg* net, const float* params, const
                                int32_t M, float* grad, float* losses_out, void* workspace, dwbc_stream_t stream);
 
 /* clip_grad_norm_(max_norm) + Adam step (PPO:245-246) over params[first, first+count) of the flat
- * buffers; `step` is the 1-based Adam step of this parameter group.  norm_scratch[2] is device
- * scratch.  grad_norm_out (optional, device) receives the pre-clip total norm. */
+ * buffers; `step` is the 1-based Adam step of this parameter group.  norm_scratch[DWBC_NORM_SCRATCH]
+ * (double) is device scratch, needing no initialisation: one partial sum of squares per block, added
+ * up in block order so that the norm and the clip coefficient repeat bit for bit.  grad_norm_out
+ * (optional, device) receives the pre-clip total norm. */
+#define DWBC_NORM_SCRATCH 592
 int dwbc_clip_adam_step(float* params, float* grad, float* adam_m, float* adam_v, int64_t first, int64_t count,
                         const DwbcPpoHyper* hp, int32_t step, double* norm_scratch, float* grad_norm_out,
                         dwbc_stream_t stream);

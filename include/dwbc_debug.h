@@ -8,7 +8,9 @@ extern "C" {
 #endif
 
 /* One GEMM of the selected implementation (tc: 0 = fp32 CUDA cores, 1 = TF32 wgmma) on plain row-major device matrices.
- *   mode 0: Y[M,N] = act(X[M,K] W[N,K]^T + b)   mode 1: dX[M,N] = G[M,K] W[K,N]   mode 2: dW[M,N] += G[K,M]^T X[K,N], db += colsum(G) */
+ *   mode 0: Y[M,N] = act(X[M,K] W[N,K]^T + b)   mode 1: dX[M,N] = G[M,K] W[K,N]   mode 2: dW[M,N] += G[K,M]^T X[K,N], db += colsum(G)
+ * Mode 2 and dwbc_debug_wgrad_group take no workspace: they allocate the scratch of their fixed-order partial sums on `stream`
+ * (cudaMallocAsync) and free it behind their launches (cudaFreeAsync) -- unlike the entry points of dwbc.h, which allocate nothing. */
 int dwbc_debug_gemm(int mode, int tc, const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc,
                     const float* bias, float* dbias, int M, int N, int K, int act, dwbc_stream_t stream);
 
@@ -48,6 +50,9 @@ typedef struct {
 int dwbc_debug_wgrad_group(const DwbcWgradGemm* gemms, int n, int rows, int x3, dwbc_stream_t stream);
 /* work items per CTA of the grouped weight-gradient launch (default 4); more when items of equal cost would exceed 1024 rows */
 int dwbc_debug_set_wgrad_items(int per_cta);
+/* Floats of partial area the grouped weight-gradient launch of dwbc_ppo_minibatch_grad would need (`need`) on `sms` SMs with `items`
+ * work items per CTA, and the floats dwbc_workspace_bytes reserves for it (`bound`).  Host code, no GPU. */
+int dwbc_debug_wgrad_partials(const DwbcNetCfg* net, int32_t rows, int sms, int items, int64_t* need, int64_t* bound);
 
 #ifdef __cplusplus
 }
