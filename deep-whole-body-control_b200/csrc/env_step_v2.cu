@@ -63,14 +63,6 @@ __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.comm
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// optional phase timing (profiling aid): clock64 at phase boundaries of every CTA, [grid][8]
-__device__ unsigned long long* g_v2_cycles = nullptr;
-#ifdef DWBC_PROFILE_PHASES
-#define V2_TICK(k) do { if (g_v2_cycles && tid == 64) g_v2_cycles[blockIdx.x * 8 + (k)] = clock64(); } while (0)
-#else
-#define V2_TICK(k) do { } while (0)
-#endif
-
 // Philox stream with a one-block cache: consecutive columns share a Philox4x32-10 evaluation.
 struct RngC {
   const float* table;
@@ -220,7 +212,6 @@ env_step_v2_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant
   int* oob_s = reinterpret_cast<int*>(sm + Ly::o_oob);
   long long* ep_s = reinterpret_cast<long long*>(sm + Ly::o_eplen);
 
-  V2_TICK(0);
   // ---- 1. TMA loads ------------------------------------------------------------------------------
   if (tid == 0) {
     mbar_init(&bar, 1);
@@ -294,7 +285,6 @@ env_step_v2_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant
   }
   mbar_wait(&bar, 0);
   __syncthreads();
-  V2_TICK(1);
 
   const float c = cfg.clip_obs > 0.0f ? cfg.clip_obs : INFINITY;
   constexpr int p4 = P >> 2, pp4 = (P + NPRIV) >> 2, nh4 = HP >> 2;
@@ -369,7 +359,6 @@ env_step_v2_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant
 #undef FEAT
   }
   cbar();
-  V2_TICK(2);
 
   // ---- assembly of one env's observation columns (WG:966-1001, Appendix B): warp per env, lane per column.
   // part 0 = columns that depend only on the simulator state (joint positions / velocities, last action, foot contacts,
@@ -619,7 +608,6 @@ env_step_v2_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant
     ep_s[e] = ep;
   }
   cbar();
-  V2_TICK(3);
 
   // ---- 7. fix-up pass: rare events, one warp per flagged env ------------------------------------
   const unsigned fix_list = __ballot_sync(FULL, lane < V2_E && (flags_s[lane] & (F_GOAL_RS | F_RESET)) != 0);   // same value in every warp
@@ -709,7 +697,6 @@ env_step_v2_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant
     }
   }
   cbar();
-  V2_TICK(4);
 
   // ---- 8. assembly pass, second half: a reset env is re-assembled from its post-reset state first -------------
   for (int e = wid; e < V2_E; e += V2_CW) {
@@ -732,7 +719,6 @@ env_step_v2_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant
   }
   fence_async_smem();  // generic-proxy writes to the state rows must be visible to the bulk stores below
   cbar();
-  V2_TICK(5);
 
   // ---- 9. write-out ------------------------------------------------------------------------------
   if (tid == 0) {
@@ -791,17 +777,12 @@ env_step_v2_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant
       for (int i = lane; i < nh4; i += 32) hg4[i] = prop4[i % p4];
     }
   }
-  V2_TICK(6);
   if (tid == 0) bulk_wait_all();  // smem must stay alive until the state-row bulk stores have read it
 }
 
 }  // namespace dwbc
 
 using namespace dwbc;
-
-extern "C" int dwbc_debug_set_cycle_buffer(unsigned long long* dev_ptr) {
-  return cudaMemcpyToSymbol(g_v2_cycles, &dev_ptr, sizeof(dev_ptr)) == cudaSuccess ? DWBC_OK : DWBC_ERR_LAUNCH;
-}
 
 // launcher used by dwbc_post_physics_step (env_step.cu); DWBC_ERR_UNSUPPORTED -> caller falls back to v1
 int dwbc_launch_env_step_v2(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, const DwbcStepArgs* args, cudaStream_t st) {

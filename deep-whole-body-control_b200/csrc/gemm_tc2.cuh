@@ -103,9 +103,9 @@ __device__ __forceinline__ void t2_fill_rows_async(float* smem, const float* bas
   }
   asm volatile("cp.async.wait_all;" ::: "memory");
 }
-// transposing K-major fill (source indexed [k][mn]); optional column sums of the source into dsum (smem atomics)
+// transposing K-major fill (source indexed [k][mn])
 __device__ __forceinline__ void t2_fill_T(float* smem, const float* base, const int64_t* rowoff, int nk, int kpad, int mnvalid, int mnpad,
-                                          bool vec, int ptid, float* dsum) {
+                                          bool vec, int ptid) {
   const int chunks = mnpad >> 2, kq = kpad >> 2, cg = (chunks + 3) >> 2, total = (kpad >> 3) * cg * 32;
   for (int b0 = ptid; b0 < total; b0 += 8 * T2_PROD) {
     float4 v[8];
@@ -138,7 +138,6 @@ __device__ __forceinline__ void t2_fill_T(float* smem, const float* base, const 
       for (int j = 0; j < 4; ++j) {
         const int mn = 4 * cc[u] + j;
         smem[((size_t)((mn >> 3) * kq + (k >> 2)) * 8 + (mn & 7)) * 4 + (k & 3)] = vv[j];
-        if (dsum && mn < mnvalid) atomicAdd(dsum + mn, vv[j]);
       }
     }
   }
@@ -176,7 +175,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) gemm_tc2_kernel(const GemmArgs 
     } else {
       for (int r = ptid; r < 128; r += T2_PROD) sh.rowoff[r] = g.B.row(r < K ? r : 0) - g.B.p;
       t2_pbar();
-      t2_fill_T(sB, g.B.p, sh.rowoff, K, kpad, N, npad, vecB & 1, ptid, nullptr);
+      t2_fill_T(sB, g.B.p, sh.rowoff, K, kpad, N, npad, vecB & 1, ptid);
     }
     for (int j = 0; j < my_items; ++j) {
       const int it = blockIdx.x + j * gridDim.x, s = j & 1;
@@ -186,10 +185,8 @@ __global__ void __launch_bounds__(T2_THREADS, 1) gemm_tc2_kernel(const GemmArgs 
       if (ptid < TC_M) sh.rowoff[ptid] = ptid < rows ? (g.A.row(m0 + ptid) - g.A.p) : 0;
       tc_mbar_wait(&sh.empty[s], ((j >> 1) & 1) ^ 1);   // stage free (epilogue of tile j-2 done)
       t2_pbar();
-      if (!(vecA & 2)) {
-        if ((vecA & 1) && (K & 3) == 0) t2_fill_rows_async(sA[s], g.A.p, sh.rowoff, rows, TC_M, K, kpad, ptid);
-        else t2_fill_rows(sA[s], g.A.p, sh.rowoff, rows, TC_M, K, kpad, vecA & 1, ptid);
-      }
+      if ((vecA & 1) && (K & 3) == 0) t2_fill_rows_async(sA[s], g.A.p, sh.rowoff, rows, TC_M, K, kpad, ptid);
+      else t2_fill_rows(sA[s], g.A.p, sh.rowoff, rows, TC_M, K, kpad, vecA & 1, ptid);
       tc_fence_async_smem();                            // generic-proxy operand writes -> async-proxy reads of the wgmma
       t2_arrive(&sh.full[s]);
       if (ptid == 0) T2_STAMP(2 + j);
@@ -231,7 +228,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) gemm_tc2_kernel(const GemmArgs 
       }
       t2_ebar();
       if (tid == T2_PROD) T2_STAMP(17 + 4 * j);
-      if (!(vecB & 2) && n4 < N) {
+      if (n4 < N) {
         const bool full = n4 + 3 < N;
         for (int r0 = ew; r0 < rows; r0 += 16) {          // 4 independent rows per iteration (ILP over the dependent exp / store chains)
           float x[4][4], y[4][4];
@@ -263,15 +260,14 @@ __global__ void __launch_bounds__(T2_THREADS, 1) gemm_tc2_kernel(const GemmArgs 
               float tt = x[u][qq];
               if (kMode == GEMM_FWD) {
                 tt += bias4[qq];
-                if (vecB & 8) { }
-                else tt = act_f<true>(g.act, tt);   // ex2.approx: 2 ulp, far below the TF32 input rounding
+                tt = act_f<true>(g.act, tt);   // ex2.approx: 2 ulp, far below the TF32 input rounding
               } else if (g.act != ACT_NONE) tt *= act_df(g.act, y[u][qq]);
               x[u][qq] = tt;
             }
           }
 #pragma unroll
           for (int u = 0; u < 4; ++u) {
-            if (!ok[u] || (vecB & 4)) continue;
+            if (!ok[u]) continue;
             float* crow = g.C + (m0 + r0 + 4 * u) * g.ldc + n4;
             if (full && c_al) *reinterpret_cast<float4*>(crow) = make_float4(x[u][0], x[u][1], x[u][2], x[u][3]);
             else for (int qq = 0; qq < 4; ++qq) if (n4 + qq < N) crow[qq] = x[u][qq];
@@ -284,8 +280,6 @@ __global__ void __launch_bounds__(T2_THREADS, 1) gemm_tc2_kernel(const GemmArgs 
     }
   }
 }
-
-extern int tc_debug;   // profiling switches: 2 = skip A fills, 4 = skip epilogue global traffic (results invalid)
 
 template <int kMode>
 inline int launch_gemm_tc2(const GemmArgs& g_in, cudaStream_t st) {
@@ -305,7 +299,7 @@ inline int launch_gemm_tc2(const GemmArgs& g_in, cudaStream_t st) {
     if (cudaFuncSetAttribute(gemm_tc2_kernel<kMode>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return DWBC_ERR_LAUNCH;
     attr[kMode] = true;
   }
-  gemm_tc2_kernel<kMode><<<grid, T2_THREADS, smem, st>>>(g, items, (rowmat_vec_ok(g.A) ? 1 : 0) | (tc_debug & 2), (rowmat_vec_ok(g.B) ? 1 : 0) | ((tc_debug & 4) >> 1) | ((tc_debug & 24) >> 1));
+  gemm_tc2_kernel<kMode><<<grid, T2_THREADS, smem, st>>>(g, items, rowmat_vec_ok(g.A) ? 1 : 0, rowmat_vec_ok(g.B) ? 1 : 0);
   ++dwbc_launch_counter;
   return cudaGetLastError() == cudaSuccess ? DWBC_OK : DWBC_ERR_LAUNCH;
 }

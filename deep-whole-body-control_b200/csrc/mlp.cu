@@ -26,7 +26,6 @@ thread_local int mlp_act = 0;
 // partial area of the weight-gradient launches of the CURRENT call (gemm_simt.cuh): the workspace's, set by make_plan
 thread_local float* mlp_wpart = nullptr;
 thread_local int64_t mlp_wpart_cap = 0;
-int tc_debug = 0;
 
 static inline int64_t align_up(int64_t x, int64_t a) { return (x + a - 1) / a * a; }
 
@@ -137,8 +136,8 @@ static int64_t loss_part_floats(int64_t rows) {
   return (rows + 127) / 128 * C2_WORKERS * C2_FIN_PART;
 }
 
-// Partials of the weight-gradient launches, for every plan a call with `rows` rows can make (any SM count, any dwbc_debug_set_wgrad_items),
-// and never fewer for more rows: the largest of
+// Partials of the weight-gradient launches, for every plan a call with `rows` rows can make (any SM count), and
+// never fewer for more rows: the largest of
 //   the grouped launch: at most wg_max_nslab(rows) slabs per GEMM, and its GEMMs' slots hold at most every parameter (+ alignment);
 //   one layer-wise TF32 weight gradient (<= 128 x 128) over at most rows x num_hist rows (the history projection);
 //   one split-K CUDA-core weight gradient: CTAs x splits < tiles + 592, tiles <= (d / 64)^2 for the widest operand d.
@@ -1017,7 +1016,7 @@ extern "C" int dwbc_ppo_minibatch_grad(const DwbcNetCfg* net, const float* param
     f.ts_w = hp->torque_supervision_weight;
     TRY(launch_pack2(ch.pl, st));
     TRY(launch_chain2(&ch.b[0].pr, &ch.b[1].pr, f, x3, p.queue, st));
-    TRY(launch_chain2(&ch.b[2].pr, &ch.b[3].pr, FinArgs{}, x3, p.queue, st, c2_bwd_reverse != 0));
+    TRY(launch_chain2(&ch.b[2].pr, &ch.b[3].pr, FinArgs{}, x3, p.queue, st, true));      // downwards: the last tiles are still in L2
     return weight_gradients(n, grad, s, idx, rows, p, st);
   }
   TRY(priv_forward(n, P, s->observations, idx, s->obs_stride, rows, p, st));
@@ -1187,12 +1186,6 @@ extern "C" int dwbc_debug_gemm(int mode, int tc, const float* A, int64_t lda, co
   return rc;
 }
 
-// tuning aid (tools/update_timing.py): time ratio of a one-tile chain item to half a two-tile item in the work-item planner; <= 0 switches
-// the one-tile tail items off
-extern "C" int dwbc_debug_set_chain_single_penalty(double v) {
-  c2_single_penalty = v;
-  return DWBC_OK;
-}
 // The chain PROGRAMS a call would launch, described without launching anything (host code only, no GPU; every pointer is formed from the
 // fake bases below and never dereferenced).  what: 0 = dwbc_policy_act, 1 = dwbc_critic_values, 2 = forward + loss of dwbc_ppo_minibatch_grad,
 // 3 = its backward launch.  out = [nprog, pack items, then per program: n_ops, n_loads, then per op: N, kpad, act, fin, fin_c, out_col0,
@@ -1235,19 +1228,6 @@ extern "C" int dwbc_debug_chain_plan(int tiles, int nprog, const double* cost, i
   if (span0) *span0 = c2_makespan(tiles, nprog, cost, sms, 0);
   return DWBC_OK;
 }
-// tuning aid: deal of the grouped weight-gradient work items (1 = sorted + boustrophedon, 0 = round-robin in construction order)
-extern "C" int dwbc_debug_set_wgrad_snake(int on) {
-  wg_snake = on ? 1 : 0;
-  return DWBC_OK;
-}
-extern "C" int dwbc_debug_set_chain_bwd_reverse(int on) {
-  c2_bwd_reverse = on ? 1 : 0;
-  return DWBC_OK;
-}
-extern "C" int dwbc_debug_set_wgrad_reverse(int on) {
-  wg_reverse = on ? 1 : 0;
-  return DWBC_OK;
-}
 // The grouped weight-gradient launch on caller-described GEMMs (tests/test_gpu_wgrad_group.py)
 extern "C" int dwbc_debug_wgrad_group(const DwbcWgradGemm* gemms, int n, int rows, int x3, dwbc_stream_t stream) {
   if (!gemms || n <= 0 || n > WG_MAX || rows <= 0) return DWBC_ERR_ARG;
@@ -1266,25 +1246,15 @@ extern "C" int dwbc_debug_wgrad_group(const DwbcWgradGemm* gemms, int n, int row
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   return with_debug_wpart(wg_max_nslab(rows) * slots, st, [&] { return launch_wgrad_group(b.g, rows, x3 != 0, st); });
 }
-extern "C" int dwbc_debug_set_wgrad_items(int per_cta) {
-  if (per_cta < 1 || per_cta > 64) return DWBC_ERR_ARG;
-  wg_items_per_cta = per_cta;
-  return DWBC_OK;
-}
-// tuning aid: force the number of one-tile items per program of the large chain launches (-1: planner)
-extern "C" int dwbc_debug_set_chain_singles(int n) {
-  c2_force_singles = n;
-  return DWBC_OK;
-}
 extern "C" int dwbc_debug_set_tc_cycle_buffer(unsigned long long* dev_ptr) {
   return cudaMemcpyToSymbol(g_tc_cycles, &dev_ptr, sizeof(dev_ptr)) == cudaSuccess ? DWBC_OK : DWBC_ERR_LAUNCH;
 }
 
-// The partial area the grouped weight-gradient launch of dwbc_ppo_minibatch_grad would use on `sms` SMs with `items` per CTA, and the
-// area dwbc_workspace_bytes reserves for it (host code only, no GPU; tests/test_reproducibility_cpu.py checks need <= bound)
-extern "C" int dwbc_debug_wgrad_partials(const DwbcNetCfg* net, int32_t rows, int sms, int items, int64_t* need, int64_t* bound) {
+// The partial area the grouped weight-gradient launch of dwbc_ppo_minibatch_grad would use on `sms` SMs, and the area
+// dwbc_workspace_bytes reserves for it (host code only, no GPU; tests/test_reproducibility_cpu.py checks need <= bound)
+extern "C" int dwbc_debug_wgrad_partial_floats(const DwbcNetCfg* net, int32_t rows, int sms, int64_t* need, int64_t* bound) {
   TRY(check_net(net));
-  if (rows <= 0 || sms <= 0 || items < 1 || items > 64 || !need || !bound) return DWBC_ERR_ARG;
+  if (rows <= 0 || sms <= 0 || !need || !bound) return DWBC_ERR_ARG;
   float* const ws = reinterpret_cast<float*>(uintptr_t(1) << 40);
   DwbcStorage s{};
   s.observations = reinterpret_cast<const float*>(uintptr_t(2) << 40);
@@ -1294,7 +1264,7 @@ extern "C" int dwbc_debug_wgrad_partials(const DwbcNetCfg* net, int32_t rows, in
   mlp_wpart_cap = 0;
   WGroupBuilder wb;
   if (!wgrad_gemms(wb, *net, ws, &s, reinterpret_cast<const int64_t*>(uintptr_t(3) << 40), p)) return DWBC_ERR_UNSUPPORTED;
-  *need = wg_plan(wb.g, rows, mlp_precision == 2, sms, items);
+  *need = wg_plan(wb.g, rows, mlp_precision == 2, sms);
   *bound = wpart_floats(*net, rows);
   return DWBC_OK;
 }

@@ -934,7 +934,7 @@ struct C2Builder {
 // only: factor c2_single_penalty, an estimate), but they fill the tail.  The number of them is chosen by simulating the
 // queue (greedy: a CTA that becomes free takes the next item) with a per-op cost model of the epilogue-bound kernel; the choice depends
 // only on (tiles, programs), so it is cached.
-inline double c2_single_penalty = 1.35;                  // time of a one-tile item / half the time of a two-tile item; <= 0: no one-tile items
+constexpr double c2_single_penalty = 1.35;               // time of a one-tile item / half the time of a two-tile item
 inline double c2_prog_cost(const C2Prog& pr) {
   double c = 0.0;
   for (int i = 0; i < pr.n_ops; ++i) c += 0.3 + (double)pr.op[i].npad / 128.0;       // fixed hand-over + epilogue work ~ output chunks
@@ -948,29 +948,21 @@ inline double c2_makespan(int tiles, int nprog, const double* cost, int sms, int
     std::push_heap(heap.begin(), heap.end(), std::greater<double>());
   };
   const int np2 = (tiles - ns1 + 1) / 2;
-  const double pen = c2_single_penalty > 0.0 ? c2_single_penalty : 1.35;
   for (int p = 0; p < nprog; ++p)
-    for (int j = 0; j < np2; ++j) take(2 * j + 1 < tiles - ns1 ? cost[p] : 0.5 * pen * cost[p]);   // (an odd last pair holds one tile)
+    for (int j = 0; j < np2; ++j) take(2 * j + 1 < tiles - ns1 ? cost[p] : 0.5 * c2_single_penalty * cost[p]);   // (an odd last pair holds one tile)
   for (int p = 0; p < nprog; ++p)
-    for (int j = 0; j < ns1; ++j) take(0.5 * pen * cost[p]);
+    for (int j = 0; j < ns1; ++j) take(0.5 * c2_single_penalty * cost[p]);
   return *std::max_element(heap.begin(), heap.end());
 }
-inline int c2_force_singles = -1;                         // tuning aid: >= 0 overrides the planner (rounded so that whole pairs stay in front)
 inline int c2_pick_singles(int tiles, int nprog, const double* cost, int sms) {
-  if (c2_force_singles >= 0) {
-    int s1 = c2_force_singles < tiles ? c2_force_singles : tiles;
-    if (s1 > 0 && ((tiles - s1) & 1)) s1 += s1 < tiles ? 1 : -1;
-    return s1;
-  }
-  if (c2_single_penalty <= 0.0) return 0;
-  struct Key { int tiles, nprog, sms; double c0, c1, pen; int ns1; };       // (c1: the sum of the other programs' costs)
+  struct Key { int tiles, nprog, sms; double c0, c1; int ns1; };            // (c1: the sum of the other programs' costs)
   static thread_local Key cache[8];
   static thread_local int ncache = 0;
   double rest = 0.0;
   for (int k = 1; k < nprog; ++k) rest += cost[k] * (1.0 + 1e-3 * k);
   for (int i = 0; i < ncache; ++i) {
     const Key& k = cache[i];
-    if (k.tiles == tiles && k.nprog == nprog && k.sms == sms && k.c0 == cost[0] && k.c1 == rest && k.pen == c2_single_penalty) return k.ns1;
+    if (k.tiles == tiles && k.nprog == nprog && k.sms == sms && k.c0 == cost[0] && k.c1 == rest) return k.ns1;
   }
   int best = 0;
   double best_t = c2_makespan(tiles, nprog, cost, sms, 0);
@@ -979,7 +971,7 @@ inline int c2_pick_singles(int tiles, int nprog, const double* cost, int sms) {
     if (t < best_t * (1.0 - 1e-9)) { best_t = t; best = s1; }
   }
   Key& k = cache[ncache < 8 ? ncache++ : 7];
-  k = Key{tiles, nprog, sms, cost[0], rest, c2_single_penalty, best};
+  k = Key{tiles, nprog, sms, cost[0], rest, best};
   return best;
 }
 
@@ -993,7 +985,6 @@ inline int c2_sm_count() {
   return sms;
 }
 
-inline int c2_bwd_reverse = 1;                            // tuning aid (dwbc_debug_set_chain_bwd_reverse): the backward launch walks the tiles downwards
 inline int launch_chain2n(const C2Prog* const* prs, int nprog, const FinArgs& fin, bool x3, int* queue, cudaStream_t st, bool rev = false);
 inline int launch_chain2(const C2Prog* pr0, const C2Prog* pr1, const FinArgs& fin, bool x3, int* queue, cudaStream_t st, bool rev = false) {
   const C2Prog* prs[2] = {pr0, pr1};
@@ -1017,10 +1008,6 @@ inline int launch_chain2n(const C2Prog* const* prs, int nprog, const FinArgs& fi
     if (pr.M <= 0 || pr.M != L.p[0].M || pr.n_ops <= 0 || pr.n_ops > C2_MAX_OPS || pr.n_loads < 0 || pr.n_loads > C2_MAX_LOADS) return DWBC_ERR_ARG;
   }
   if (!queue) return DWBC_ERR_ARG;
-#ifdef DWBC_C2_DROP_STORES      // timing experiments only (results invalid): no global activation stores
-  for (int k = 0; k < L.nprog; ++k)
-    for (int i = 0; i < L.p[k].n_ops; ++i) L.p[k].op[i].y = nullptr;
-#endif
   const int sms = c2_sm_count();
   const int tiles = (L.p[0].M + TC_M - 1) / TC_M;
   if (tiles * L.nprog <= sms || x3) {                      // small batches (rollout): one tile per item, spread over more SMs; 3xTF32: the

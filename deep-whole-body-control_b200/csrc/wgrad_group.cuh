@@ -38,11 +38,10 @@ struct WGItem {
   int64_t part;         // slot of slab 0 in the partial area; slab s at part + s * wg_slot(Mo, Ni): [Mo x Ni] dW, then [Mo] db
 };
 inline __host__ __device__ int64_t wg_slot(int Mo, int Ni) { return ((int64_t)Mo * Ni + Mo + 3) & ~(int64_t)3; }
-// Work items are enumerated GEMM by GEMM, GEMMs in the order launch_wgrad_group sorted them (longest item first).
-// snake == 0: item e goes to CTA e % grid (round-robin); snake != 0: round j of the deal runs forwards for even j, backwards for odd j.
-// Slab s of a GEMM with n slabs covers rows [b(s), b(s + 1)), b(s) = floor(s rows / n) rounded down to a whole chunk, b(n) = rows.
-// rev != 0: the slabs of a GEMM are taken from the LAST rows to the first.
-struct WGroup { int n, rows, items, snake, rev; float* part; WGItem it[WG_MAX]; };
+// Work items are enumerated GEMM by GEMM, GEMMs in the order launch_wgrad_group sorted them (longest item first), and item e goes to
+// CTA e % grid (round-robin).  Item first + s of a GEMM with n slabs is its slab s, which covers rows [b(s), b(s + 1)),
+// b(s) = floor(s rows / n) rounded down to a whole chunk, b(n) = rows.
+struct WGroup { int n, rows, items; float* part; WGItem it[WG_MAX]; };
 
 __device__ __forceinline__ void wg_cp16(float* dst, const float* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(tc_smem_u32(dst)), "l"(src) : "memory");
@@ -218,14 +217,12 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_group_kernel(const __grid
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);      // warp-uniform for ptxas: the wgmma control flow depends on it
   const int nb = (int)gridDim.x, bid = (int)blockIdx.x;
   const int items = grp.items, full = items / nb, rem = items - full * nb;
-  const int my_items = grp.snake ? full + ((((full & 1) ? nb - 1 - bid : bid) < rem) ? 1 : 0) : full + (bid < rem ? 1 : 0);
-  for (int j = 0; j < my_items; ++j) {
-    const int e = j * nb + ((grp.snake && (j & 1)) ? nb - 1 - bid : bid);
+  const int my_items = full + (bid < rem ? 1 : 0);
+  for (int j = 0, e = bid; j < my_items; ++j, e += nb) {
     int li = 0;
     while (li + 1 < grp.n && e >= grp.it[li + 1].first) ++li;
     const WGItem& g = grp.it[li];
-    int slab_i = e - g.first;
-    if (grp.rev) slab_i = g.nslab - 1 - slab_i;
+    const int slab_i = e - g.first;
     const int64_t k_begin = (int64_t)slab_i * grp.rows / g.nslab / WG_KC * WG_KC;
     const int64_t k_end = slab_i + 1 == g.nslab ? (int64_t)grp.rows : (int64_t)(slab_i + 1) * grp.rows / g.nslab / WG_KC * WG_KC;
     if (k_end <= k_begin) continue;
@@ -250,15 +247,13 @@ struct WGroupBuilder {
 // Longest slab: the accumulator sums a slab's rows in registers, and longer sums lose accuracy against the fp32 reference
 constexpr int64_t WG_MAX_SLAB = 1024;
 // Most slabs of one GEMM: the fewer of one per four chunks and WG_MAX_NSLAB, unless rows / WG_MAX_SLAB needs more.  It bounds the
-// partial area by wg_max_nslab(rows) x the GEMMs' slots, whatever the SM count and the items per CTA (dwbc_workspace_bytes).
+// partial area by wg_max_nslab(rows) x the GEMMs' slots, whatever the SM count (dwbc_workspace_bytes).
 constexpr int64_t WG_MAX_NSLAB = 128;
 inline int64_t wg_max_nslab(int64_t rows) {
   const int64_t lo = (rows + WG_MAX_SLAB - WG_KC - 1) / (WG_MAX_SLAB - WG_KC);
   return std::max<int64_t>(1, std::min(rows / (4 * WG_KC), std::max(lo, WG_MAX_NSLAB)));
 }
-inline int wg_items_per_cta = 4;                     // tuning aid (dwbc_debug_set_wgrad_items)
-inline int wg_reverse = 0;                            // tuning aid (dwbc_debug_set_wgrad_reverse): 0 = slabs from the first rows upwards
-inline int wg_snake = 0;                             // tuning aid (dwbc_debug_set_wgrad_snake): 0 = round-robin deal
+constexpr int WG_ITEMS_PER_CTA = 4;                   // fewest work items per SM
 
 // Time of one row of a GEMM on the H100 roofline: the operand bytes at 3.35 TB/s or the tensor work padded to the instruction widths
 // at 495 TFLOP/s (three products in 3xTF32 mode), whichever is larger.  Only the ratios between GEMMs matter.
@@ -270,13 +265,13 @@ inline double wg_row_cost(const WGItem& it, bool x3) {
   return std::max(bytes / 3.35e12, flop / 495e12);
 }
 
-// Plan: work items of equal cost, a whole number per CTA.  There are wg_items_per_cta per SM, or more when an item of that cost would be
+// Plan: work items of equal cost, a whole number per CTA.  There are WG_ITEMS_PER_CTA per SM, or more when an item of that cost would be
 // longer than WG_MAX_SLAB rows of the cheapest GEMM.  Each GEMM gets a number of slabs proportional to its row cost (largest remainder,
 // at least rows / WG_MAX_SLAB, at most one per four chunks), so its slabs are the shorter the more a row costs.  The GEMMs are then ordered
 // by the cost of one of their items, longest first, so that items rounded short fill the end of the launch.  At small row counts the
 // limits leave fewer items.
-// The plan on `sms` SMs with `items_per_cta` (host code); returns the floats of partial area it needs.
-inline int64_t wg_plan(WGroup& g, int rows, bool x3, int sms, int items_per_cta) {
+// The plan on `sms` SMs (host code); returns the floats of partial area it needs.
+inline int64_t wg_plan(WGroup& g, int rows, bool x3, int sms) {
   g.rows = rows;
   double cost[WG_MAX], total = 0.0, cmin = 1e30;
   for (int i = 0; i < g.n; ++i) {
@@ -284,7 +279,7 @@ inline int64_t wg_plan(WGroup& g, int rows, bool x3, int sms, int items_per_cta)
     cmin = std::min(cmin, cost[i]);
   }
   const int64_t span = WG_MAX_SLAB - WG_KC;           // rows / n, before the slab bounds are rounded down to whole chunks
-  const int64_t per_cta = std::max<int64_t>(items_per_cta, (int64_t)std::ceil((double)rows * total / ((double)sms * span * cmin) - 1e-9));
+  const int64_t per_cta = std::max<int64_t>(WG_ITEMS_PER_CTA, (int64_t)std::ceil((double)rows * total / ((double)sms * span * cmin) - 1e-9));
   const int64_t target = per_cta * sms;
   const int64_t lo = (rows + span - 1) / span, hi = wg_max_nslab(rows);
   int64_t n[WG_MAX], sum = 0;
@@ -328,15 +323,13 @@ inline int64_t wg_plan(WGroup& g, int rows, bool x3, int sms, int items_per_cta)
 
 inline int launch_wgrad_group(WGroup& g, int rows, bool x3, cudaStream_t st) {
   if (g.n <= 0 || rows <= 0) return DWBC_ERR_ARG;
-  g.snake = wg_snake;
-  g.rev = wg_reverse;
   static int sms = 0;
   if (!sms) {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   }
-  const int64_t need = wg_plan(g, rows, x3, sms, wg_items_per_cta);
+  const int64_t need = wg_plan(g, rows, x3, sms);
   const int items = g.items;
   g.part = mlp_wpart;
   if (!g.part || need > mlp_wpart_cap || (reinterpret_cast<uintptr_t>(g.part) & 15)) return DWBC_ERR_ARG;

@@ -11,7 +11,7 @@
  *
  * Conventions: every pointer is a DEVICE pointer into a caller-owned, contiguous, row-major
  * buffer (fp32 unless the type says otherwise).  The library allocates nothing, keeps no
- * global state (except a launch counter and the tuning defaults of include/dwbc_debug.h), never synchronises and never throws: every function enqueues its kernels on
+ * global state (except a launch counter and the clock-stamp pointer of dwbc_debug_set_tc_cycle_buffer), never synchronises and never throws: every function enqueues its kernels on
  * the given stream and returns DWBC_OK or a negative error code.  Structs are passed by
  * pointer to HOST memory and are read before the call returns.
  */

@@ -28,7 +28,7 @@ def test_library_exports_every_declared_symbol(lib):
 
 
 def test_debug_header_symbols_are_exported(lib):
-    """include/dwbc_debug.h (profiling / tuning hooks, outside the drop-in boundary): every declared symbol exists, and the library
+    """include/dwbc_debug.h (profiling and test hooks, outside the drop-in boundary): every declared symbol exists, and the library
     exports no dwbc_* symbol that neither header declares."""
     import subprocess
     dbg = open(os.path.join(ROOT, "include", "dwbc_debug.h")).read()

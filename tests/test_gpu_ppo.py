@@ -436,42 +436,28 @@ def test_fused_chain_forward_matches_fp32_path_many_tiles(hist, precision):
     assert all(torch.isfinite(t).all() for t in out[precision])
 
 
-@pytest.mark.parametrize("singles,snake,rev", [(-1, 0, 1), (0, 0, 0), (37, 1, 1), (-1, 1, 0)])
+# Row counts of the backward test below, one per tail shape of its tf32 chain launches on a 132-SM H100 (3xTF32 always runs one-tile
+# items).  Each is the planner's own choice (launch_chain2n) for the forward and the backward launch; test_host_cpu.py checks that it
+# stays so.  The last tile is ragged (77 rows) throughout.
+CHAIN_TAIL_ROWS = {
+    "one_tile_items": 65 * 128 + 77,                # 66 tiles x 2 programs fit the SMs: one tile per item
+    "pairs_odd_last_pair": 240 * 128 + 77,          # 241 tiles, two-tile items only: the last pair holds the ragged tile alone
+    "pairs_ragged_last_pair": 241 * 128 + 77,       # 242 tiles, two-tile items only: the ragged tile is the last pair's second
+    "one_tile_tail": 298 * 128 + 77,                # 299 tiles: 120 pairs, then 59 one-tile items, the ragged tile last
+}
+
+
+@pytest.mark.parametrize("shape", sorted(CHAIN_TAIL_ROWS))
 @pytest.mark.parametrize("precision", ["tf32", "tf32x3"])
-def test_fused_chain_backward_matches_fp32_path_many_tiles(precision, singles, snake, rev):
+def test_fused_chain_backward_matches_fp32_path_many_tiles(precision, shape):
     """Mini-batch gradient through the fused forward chains (loss in the epilogue), backward chains and the MN-major weight-gradient GEMMs
-    against the exact-fp32 layer-wise path of the same library, at a row count that gives every CTA several tile pairs plus a ragged one.
-    Tolerances: CHAIN_TOL, per parameter tensor ||g - g_fp32|| <= tol ||g_fp32|| (+ 1e-7 abs).
-    `singles`: one-tile work items per program at the tail of the chain launches (-1: the planner of launch_chain2 decides, 0: two-tile
-    items only -- the odd last pair then holds one tile --, 37: forced, the ragged last tile runs as a one-tile item); `snake`: deal of
-    the grouped weight-gradient work items (1: sorted by operand width, boustrophedon; 0: round-robin in construction order); `rev`: its
-    slab order (1: from the last rows downwards; 0: upwards, the default); the backward chain launch walks the tiles the other way round
-    (dwbc_debug_set_chain_bwd_reverse: downwards by default, after the forward launch that walked upwards)."""
-    import ctypes as C
-    from dwbc_b200 import _lib as L
-    L.lib().dwbc_debug_set_chain_singles.argtypes = [C.c_int]
-    L.lib().dwbc_debug_set_wgrad_snake.argtypes = [C.c_int]
-    L.lib().dwbc_debug_set_chain_singles(singles)
-    L.lib().dwbc_debug_set_wgrad_snake(snake)
-    L.lib().dwbc_debug_set_wgrad_reverse.argtypes = [C.c_int]
-    L.lib().dwbc_debug_set_wgrad_reverse(rev)
-    L.lib().dwbc_debug_set_chain_bwd_reverse.argtypes = [C.c_int]
-    L.lib().dwbc_debug_set_chain_bwd_reverse(1 - rev)
-    try:
-        _chain_backward_many_tiles(precision)
-    finally:
-        L.lib().dwbc_debug_set_chain_singles(-1)
-        L.lib().dwbc_debug_set_wgrad_snake(0)
-        L.lib().dwbc_debug_set_wgrad_reverse(0)
-        L.lib().dwbc_debug_set_chain_bwd_reverse(1)
-
-
-def _chain_backward_many_tiles(precision):
+    against the exact-fp32 layer-wise path of the same library, at the row counts of CHAIN_TAIL_ROWS.
+    Tolerances: CHAIN_TOL, per parameter tensor ||g - g_fp32|| <= tol ||g_fp32|| (+ 1e-7 abs)."""
     import ctypes as C
     from dwbc_b200 import _lib as L
     g = np.load(os.path.join(G, "ppo.npz"))
     P = golden_params(g, int(g["meta"][2]))
-    N, T = 148 * 128 * 2 + 333, 1
+    N, T = CHAIN_TAIL_ROWS[shape], 1
     grads, losses = {}, {}
     gen = torch.Generator(device="cuda").manual_seed(9)
     alg = make_alg(N, T, P, num_mini_batches=1, num_learning_epochs=1)

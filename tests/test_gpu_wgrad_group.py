@@ -102,21 +102,6 @@ def _run(spec, rows, x3, seed=0):
             assert float((db.double() - dbref).norm()) <= DB_TOL * float(dbscale.norm()), what
 
 
-@pytest.fixture
-def hooks():
-    from dwbc_b200 import _lib as L
-    lib = L.lib()
-    for f in ("dwbc_debug_set_wgrad_snake", "dwbc_debug_set_wgrad_reverse", "dwbc_debug_set_wgrad_items"):
-        getattr(lib, f).argtypes = [C.c_int]
-
-    def set_(snake, rev, items):
-        assert lib.dwbc_debug_set_wgrad_snake(snake) == 0
-        assert lib.dwbc_debug_set_wgrad_reverse(rev) == 0
-        assert lib.dwbc_debug_set_wgrad_items(items) == 0
-    yield set_
-    set_(0, 0, 4)
-
-
 @pytest.mark.parametrize("x3", [1, 0])
 @pytest.mark.parametrize("rows", [1, 63, 64, 129])
 def test_one_narrow_gemm_fewer_items_than_sms(rows, x3):
@@ -134,12 +119,3 @@ def test_two_gemms_image_operands(rows, x3):
 @pytest.mark.parametrize("n,rows", [(17, 40960), (17, 132 * 128 + 77), (20, 132 * 128 + 77), (20, 333)])
 def test_many_gemms_mixed_widths_and_layouts(n, rows, x3):
     _run(_spec(n, n), rows, x3, seed=n)
-
-
-@pytest.mark.parametrize("x3", [1, 0])
-@pytest.mark.parametrize("snake", [0, 1])
-@pytest.mark.parametrize("rev", [0, 1])
-@pytest.mark.parametrize("items", [1, 4, 16])
-def test_every_combination_of_the_tuning_hooks(hooks, items, rev, snake, x3):
-    hooks(snake, rev, items)
-    _run(_spec(17, 2), 132 * 128 + 77, x3, seed=3)

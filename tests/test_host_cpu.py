@@ -103,6 +103,34 @@ def test_chain_work_item_planner_host_logic():
     assert lib.dwbc_debug_chain_plan(0, 2, None, 148, None, None, None, None) == -1
 
 
+def test_backward_test_rows_get_their_chain_tail_shapes():
+    """Each row count of test_gpu_ppo.py's CHAIN_TAIL_ROWS gets the tail shape it is named for, in the tf32 forward and backward chain
+    launches of dwbc_ppo_minibatch_grad on 132 SMs: the programs from dwbc_debug_describe_chain, their costs as c2_prog_cost
+    (mlp_chain2.cuh) adds them up, longest program first as launch_chain2n queues them, the items from dwbc_debug_chain_plan."""
+    import ctypes as C
+    from dwbc_b200 import _lib as L
+    from test_chain_shapes_cpu import describe, make_ac
+    from test_gpu_ppo import CHAIN_TAIL_ROWS
+    lib = L.lib()
+    lib.dwbc_debug_chain_plan.argtypes = [C.c_int, C.c_int, C.POINTER(C.c_double), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                          C.POINTER(C.c_double), C.POINTER(C.c_double)]
+    ac = make_ac("S", "cpu")
+    for shape, rows in CHAIN_TAIL_ROWS.items():
+        tiles = (rows + 127) // 128
+        assert rows % 128
+        for what in (2, 3):
+            _, progs = describe(ac, rows, what, precision=L.PRECISIONS["tf32"], sms=132)
+            progs = sorted(progs, key=lambda q: -len(q[1]))
+            cost = [sum(0.3 + ((o["N"] + 15) & ~15) / 128.0 for o in ops) + 0.3 * n_loads for n_loads, ops in progs]
+            assert len(cost) == 2
+            c = (C.c_double * 4)(*cost)
+            np2, ns1 = C.c_int(), C.c_int()
+            assert lib.dwbc_debug_chain_plan(tiles, len(cost), c, 132, C.byref(np2), C.byref(ns1), None, None) == 0
+            got = ("one_tile_items" if np2.value == 0 else "one_tile_tail" if ns1.value else
+                   "pairs_odd_last_pair" if tiles % 2 else "pairs_ragged_last_pair")
+            assert got == shape, (shape, rows, what, np2.value, ns1.value)
+
+
 def test_chain_programs_host_logic():
     """The layer-chain PROGRAMS the entry points build (mlp.cu: build_forward / build_backward; host code, described by
     dwbc_debug_describe_chain without a GPU): a 4096-row rollout is four programs, one per head, of at most 6 ops (AC:204-217, 280-286); above

@@ -24,7 +24,7 @@ for mode in (0, 1, 2):
             for i in range(nbuf): run(mode, tc, i)
         e1.record(); torch.cuda.synchronize()
         out[f"mode{mode}_tc{tc}"] = round(e0.elapsed_time(e1) * 1e3 / (3 * nbuf), 2)
-print(json.dumps(dict(debug=os.environ.get("DWBC_TC_DEBUG", "0"), simple=os.environ.get("DWBC_TC_SIMPLE", "0"), us=out)))
+print(json.dumps(dict(us=out)))
 if len(sys.argv) > 1 and sys.argv[1] == "stamps":
     buf = torch.zeros(148 * 64, dtype=torch.int64, device="cuda")
     lib.dwbc_debug_set_tc_cycle_buffer.argtypes = [C.c_void_p]

@@ -43,29 +43,6 @@ if __name__ == "__main__":
     main(*(sys.argv[1:2] or ["flat"]), N=int(sys.argv[2]) if len(sys.argv) > 2 else 4096)
 
 
-def phases(name="flat", N=4096):
-    """Per-phase cycle breakdown of the v2 kernel (clock64 at phase boundaries, debug hook)."""
-    import ctypes as C
-    from dwbc_b200 import _lib as L
-    p = E.make_params(name, N)
-    st = synth.initial_env_state(p, 100); st.update(synth.sim_state(p, 100, 0, rp_sigma=0.05, z_lo=0.327))
-    if p.measure_heights: st["height_samples"] = synth.height_field(p, 100)
-    env = FusedWidowGo1Core(p, "cuda:0", state=st, seed=1, sync_stats=False, generic_kernel=bool(os.environ.get("DWBC_ENV_KERNEL_V1"))); env.update_command_curriculum()
-    for _ in range(15): env.post_physics_step()
-    buf = torch.zeros(N // 32 * 8, dtype=torch.int64, device="cuda")
-    lib = L.lib(); lib.dwbc_debug_set_cycle_buffer.argtypes = [C.c_void_p]
-    lib.dwbc_debug_set_cycle_buffer(buf.data_ptr())
-    env.post_physics_step(); torch.cuda.synchronize()
-    c = buf.view(-1, 8).cpu().double()
-    d = (c[:, 1:7] - c[:, 0:6])
-    names = ["tma_wait+gather", "heights+features", "scalar", "fixup", "assembly", "writeout+patch"]
-    print({n: (round(float(d[:, i].median())), round(float(d[:, i].max()))) for i, n in enumerate(names)}, "total", float((c[:, 6] - c[:, 0]).median()))
-    lib.dwbc_debug_set_cycle_buffer(None)
-
-if __name__ == "__main__" and len(sys.argv) > 3 and sys.argv[3] == "phases":
-    phases(sys.argv[1], int(sys.argv[2]))
-
-
 def queued(name="flat", N=4096, n=40, reps=5):
     """True back-to-back kernel time: fill the stream behind a ~20 ms spin kernel, then time n launches."""
     import ctypes as C

@@ -1,4 +1,4 @@
-"""update() wall time (CUDA events, 3 repetitions) of the bench-sized storage; tuning knobs come from the environment."""
+"""update() wall time (CUDA events, 3 repetitions) of the bench-sized storage."""
 import os, sys, json
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import torch
@@ -17,4 +17,4 @@ e0.record()
 for _ in range(3):
     alg.update()
 e1.record(); torch.cuda.synchronize()
-print(json.dumps({"wg_items": os.environ.get("DWBC_WG_ITEMS", "4"), "update_ms": round(e0.elapsed_time(e1) / 3, 3)}))
+print(json.dumps({"update_ms": round(e0.elapsed_time(e1) / 3, 3)}))
