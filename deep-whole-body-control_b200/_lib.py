@@ -76,6 +76,14 @@ class StepArgs(C.Structure):
                 ("leg_termination_scale", f32), ("arm_termination_scale", f32), ("generic_kernel", i32), ("reserved_", i32)]
 
 
+class StepDevice(C.Structure):
+    """DwbcStepDevice: the per-step values dwbc_post_physics_step_device reads from device memory."""
+    _fields_ = [("step", u64), ("push_interval", i32), ("reserved_", i32),
+                ("lin_vel_x", f32 * 2), ("ang_vel_yaw", f32 * 2), ("goal_l", f32 * 2), ("goal_p", f32 * 2), ("goal_y", f32 * 2),
+                ("leg_scale", f32 * MAX_TERMS), ("arm_scale", f32 * MAX_TERMS),
+                ("leg_termination_scale", f32), ("arm_termination_scale", f32)]
+
+
 class NetCfg(C.Structure):
     _fields_ = [
         ("abi_version", i32),
@@ -146,8 +154,12 @@ _SIGS = {
     "dwbc_dagger_minibatch_grad": [vp, vp, vp, vp, i32, vp, vp, vp, vp],
     "dwbc_clip_adam_step": [vp, vp, vp, vp, i64, i64, vp, i32, vp, vp, vp],
     "dwbc_enforce_min_std": [vp, i64, vp, i32, vp],
+    "dwbc_adam_bias_correction": [vp, i32, i32, vp],
+    "dwbc_post_physics_step_device": [vp, vp, vp, vp, vp],
+    "dwbc_ppo_minibatch_grad_sched": [vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp],
+    "dwbc_clip_adam_step_table": [vp, vp, vp, vp, i64, i64, vp, i32, vp, vp, vp, vp],
 }
-EXPORTS = sorted(list(_SIGS) + ["dwbc_workspace_bytes", "dwbc_version", "dwbc_struct_sizes", "dwbc_launch_count"])
+EXPORTS = sorted(list(_SIGS) + ["dwbc_workspace_bytes", "dwbc_version", "dwbc_struct_sizes", "dwbc_launch_count", "dwbc_step_device_size"])
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
@@ -180,11 +192,13 @@ def lib():
     L.dwbc_launch_count.restype = C.c_uint64
     L.dwbc_struct_sizes.argtypes = [C.POINTER(i64 * 6)]
     L.dwbc_struct_sizes.restype = None
+    L.dwbc_step_device_size.restype = i64
     sizes = (i64 * 6)()
     L.dwbc_struct_sizes(C.byref(sizes))
     mine = [C.sizeof(s) for s in (EnvCfg, EnvBuffers, StepArgs, NetCfg, PpoHyper, Storage)]
-    if list(sizes) != mine:
-        raise DwbcError(f"struct layout mismatch between include/dwbc.h and _lib.py: C {list(sizes)} vs ctypes {mine}")
+    if list(sizes) != mine or L.dwbc_step_device_size() != C.sizeof(StepDevice):
+        raise DwbcError(f"struct layout mismatch between include/dwbc.h and _lib.py: C {list(sizes) + [L.dwbc_step_device_size()]} vs "
+                        f"ctypes {mine + [C.sizeof(StepDevice)]}")
     _lib = L
     return L
 
@@ -206,6 +220,15 @@ def ptr(t, dtype=None):
     if dtype is not None and t.dtype not in (dtype if isinstance(dtype, tuple) else (dtype,)):
         raise DwbcError(f"dwbc kernel argument has dtype {t.dtype}, expected {dtype}")
     return t.data_ptr()
+
+
+def adam_bias_correction(hp: PpoHyper, first_step: int, n: int):
+    """(lr / bc1, sqrt(bc2)) of Adam steps first_step .. first_step + n - 1 as dwbc_clip_adam_step computes them on the host: a float32
+    numpy array [n, 2], the table dwbc_clip_adam_step_table reads."""
+    import numpy as np
+    out = np.zeros((max(n, 0), 2), np.float32)
+    check(lib().dwbc_adam_bias_correction(C.addressof(hp), int(first_step), int(n), out.ctypes.data), "dwbc_adam_bias_correction")
+    return out
 
 
 def stream_ptr():

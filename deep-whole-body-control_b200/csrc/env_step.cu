@@ -635,16 +635,18 @@ __global__ void pre_physics_actions_kernel(const float* __restrict__ pol, const 
 
 using namespace dwbc;
 
-int dwbc_launch_env_step_v2(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, const DwbcStepArgs* args, cudaStream_t st);
+int dwbc_launch_env_step_v2(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, const DwbcStepArgs* args, const DwbcStepDevice* dev, cudaStream_t st);
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 // extras['episode'] of one step in a fixed order: block c adds column c of the slots of the envs that reset, in env order (thread t:
 // envs t, t + 256, ...; then a fixed tree), column 0 counting them; episode_stats[c] += that sum
+// With a device step record (dwbc_post_physics_step_device) block 0 also advances its step: the post-physics kernel before it has used it.
 __global__ void __launch_bounds__(256) episode_stats_kernel(const uint8_t* __restrict__ reset, const float* __restrict__ slots, int stride, int n,
-                                                            float* __restrict__ stats) {
+                                                            float* __restrict__ stats, DwbcStepDevice* __restrict__ dev) {
   __shared__ float red[256];
   const int c = blockIdx.x;
+  if (dev && c == 0 && threadIdx.x == 0) dev->step += 1;
   float s = 0.0f;
   for (int e = threadIdx.x; e < n; e += 256)
     if (reset[e]) s += c == 0 ? 1.0f : slots[(size_t)e * stride + c - 1];
@@ -657,15 +659,16 @@ __global__ void __launch_bounds__(256) episode_stats_kernel(const uint8_t* __res
   if (threadIdx.x == 0) stats[c] += red[0];
 }
 
-static int launch_episode_stats(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, cudaStream_t st) {
+static int launch_episode_stats(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, DwbcStepDevice* dev, cudaStream_t st) {
   episode_stats_kernel<<<1 + cfg->n_sum_slots + DWBC_NUM_METRICS, 256, 0, st>>>(buf->reset_buf, buf->episode_scratch, cfg->sums_stride,
-                                                                              cfg->num_envs, buf->episode_stats);
+                                                                              cfg->num_envs, buf->episode_stats, dev);
   DWBC_LAUNCH_CHECK();
   return DWBC_OK;
 }
 
-extern "C" int dwbc_post_physics_step(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, const DwbcStepArgs* args,
-                                      dwbc_stream_t stream) {
+// dev: optional device step record (dwbc_post_physics_step_device)
+static int post_physics_step(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, const DwbcStepArgs* args, DwbcStepDevice* dev,
+                             dwbc_stream_t stream) {
   if (!cfg || !buf || !args) return DWBC_ERR_ARG;
   if (cfg->abi_version != DWBC_ABI_VERSION || cfg->num_envs <= 0) return DWBC_ERR_ARG;
   const int nd = cfg->num_dofs, na = cfg->num_actions;
@@ -694,16 +697,28 @@ extern "C" int dwbc_post_physics_step(const DwbcEnvCfg* cfg, const DwbcEnvBuffer
       aligned16(buf->torques) && aligned16(buf->actions) && aligned16(buf->action_history) && aligned16(buf->mass_params) &&
       aligned16(buf->friction) && aligned16(buf->motor_strength) && aligned16(buf->goal_state) && aligned16(buf->derived_state) &&
       aligned16(buf->episode_length) && aligned16(buf->episode_sums) && !args->generic_kernel) {
-    const int rc = dwbc_launch_env_step_v2(cfg, buf, args, (cudaStream_t)stream);
-    if (rc != DWBC_ERR_UNSUPPORTED) return rc == DWBC_OK ? launch_episode_stats(cfg, buf, (cudaStream_t)stream) : rc;
+    const int rc = dwbc_launch_env_step_v2(cfg, buf, args, dev, (cudaStream_t)stream);
+    if (rc != DWBC_ERR_UNSUPPORTED) return rc == DWBC_OK ? launch_episode_stats(cfg, buf, dev, (cudaStream_t)stream) : rc;
   }
+  if (dev) return DWBC_ERR_UNSUPPORTED;      // the warp-per-env kernel reads the host fields only
   const int grid = (cfg->num_envs + ENV_WARPS - 1) / ENV_WARPS;
   if ((int64_t)cfg->history_len * cfg->num_prop <= MAX_H4 * 128)
     env_step_kernel<false><<<grid, ENV_WARPS * 32, 0, (cudaStream_t)stream>>>(*cfg, *buf, *args);
   else
     env_step_kernel<true><<<grid, ENV_WARPS * 32, 0, (cudaStream_t)stream>>>(*cfg, *buf, *args);
   DWBC_LAUNCH_CHECK();
-  return launch_episode_stats(cfg, buf, (cudaStream_t)stream);
+  return launch_episode_stats(cfg, buf, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int dwbc_post_physics_step(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, const DwbcStepArgs* args,
+                                      dwbc_stream_t stream) {
+  return post_physics_step(cfg, buf, args, nullptr, stream);
+}
+
+extern "C" int dwbc_post_physics_step_device(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, const DwbcStepArgs* args, DwbcStepDevice* device,
+                                             dwbc_stream_t stream) {
+  if (!device) return DWBC_ERR_ARG;
+  return post_physics_step(cfg, buf, args, device, stream);
 }
 
 extern "C" int dwbc_fill_uniform(float* out, int32_t num_envs, uint64_t seed, uint64_t step, dwbc_stream_t stream) {

@@ -134,6 +134,26 @@ struct RngW {
 };
 
 // warp-cooperative EE-goal resampling (WG:1316-1332); collision samples spread over lanes (WG:1337-1342)
+// Word `tid` of the step arguments a kernel works with: the host's DwbcStepArgs, except that with a device record (CUDA-graph replay) the
+// step, the push decision (WG:934) and the curriculum values come from that record.  Threads 0 .. sizeof(DwbcStepArgs) / 4 - 1 take part.
+static_assert(offsetof(DwbcStepArgs, generic_kernel) - offsetof(DwbcStepArgs, lin_vel_x) == sizeof(DwbcStepDevice) - offsetof(DwbcStepDevice, lin_vel_x),
+              "the curriculum block of DwbcStepDevice mirrors the one of DwbcStepArgs");
+static_assert(sizeof(DwbcStepArgs) / 4 <= V2_THREADS && sizeof(DwbcStepArgs) % 4 == 0, "one word per thread");
+__device__ __forceinline__ void step_args_to_shared(const DwbcStepArgs& h, const DwbcStepDevice* d, DwbcStepArgs* out, int tid) {
+  constexpr int NW = sizeof(DwbcStepArgs) / 4, W_STEP = offsetof(DwbcStepArgs, step) / 4, W_PUSH = offsetof(DwbcStepArgs, do_push) / 4;
+  constexpr int W_CUR0 = offsetof(DwbcStepArgs, lin_vel_x) / 4, W_CUR1 = offsetof(DwbcStepArgs, generic_kernel) / 4;
+  if (tid >= NW) return;
+  uint32_t v = reinterpret_cast<const uint32_t*>(&h)[tid];
+  if (d) {
+    const uint64_t step = d->step;
+    if (tid >= W_CUR0 && tid < W_CUR1) v = reinterpret_cast<const uint32_t*>(d->lin_vel_x)[tid - W_CUR0];
+    else if (tid == W_STEP) v = (uint32_t)step;
+    else if (tid == W_STEP + 1) v = (uint32_t)(step >> 32);
+    else if (tid == W_PUSH) v = (d->push_interval > 0 && step % (uint64_t)d->push_interval == 0) ? 1u : 0u;
+  }
+  reinterpret_cast<uint32_t*>(out)[tid] = v;
+}
+
 __device__ void coop_resample_goal(const DwbcEnvCfg& cfg, const DwbcStepArgs& A, const RngW& rng, float* gs, float yaw, int col_orn, int col_sph,
                                    bool do_orn, int lane) {
   {
@@ -192,10 +212,12 @@ __device__ void coop_resample_goal(const DwbcEnvCfg& cfg, const DwbcStepArgs& A,
 
 template <int ND, int NA, int AH, int P, int H, int NPRIV>
 __global__ void __launch_bounds__(V2_THREADS, 2)
-env_step_v2_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant__ DwbcEnvBuffers B, const __grid_constant__ DwbcStepArgs A) {
+env_step_v2_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant__ DwbcEnvBuffers B, const __grid_constant__ DwbcStepArgs Ah,
+                   const DwbcStepDevice* __restrict__ dev) {
   using Ly = V2<ND, NA, AH, P, H, NPRIV>;
   constexpr int HP = Ly::HP, CFS = Ly::CFS;
   extern __shared__ __align__(128) float sm[];
+  __shared__ DwbcStepArgs A;      // this step's arguments: the host's, or with `dev` the device record's step / push / curriculum values
   __shared__ __align__(8) uint64_t bar;
   __shared__ int cta_flags;
   __shared__ int feat_mask;
@@ -212,6 +234,7 @@ env_step_v2_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant
   int* oob_s = reinterpret_cast<int*>(sm + Ly::o_oob);
   long long* ep_s = reinterpret_cast<long long*>(sm + Ly::o_eplen);
 
+  step_args_to_shared(Ah, dev, &A, tid);   // (ordered before every use by the barrier below)
   // ---- 1. TMA loads ------------------------------------------------------------------------------
   if (tid == 0) {
     mbar_init(&bar, 1);
@@ -785,7 +808,7 @@ env_step_v2_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant
 using namespace dwbc;
 
 // launcher used by dwbc_post_physics_step (env_step.cu); DWBC_ERR_UNSUPPORTED -> caller falls back to v1
-int dwbc_launch_env_step_v2(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, const DwbcStepArgs* args, cudaStream_t st) {
+int dwbc_launch_env_step_v2(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, const DwbcStepArgs* args, const DwbcStepDevice* dev, cudaStream_t st) {
   using K = V2<20, 18, 4, 76, 10, 24>;
   if (cfg->num_dofs != 20 || cfg->num_actions != 18 || cfg->action_hist_len != 4 || cfg->num_prop != 76 || cfg->history_len != 10 ||
       cfg->num_priv != 24 || (cfg->sums_stride & 3) || cfg->n_collision_samples > 32)
@@ -798,7 +821,7 @@ int dwbc_launch_env_step_v2(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, co
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024) != cudaSuccess) return DWBC_ERR_LAUNCH;
     attr_set = true;
   }
-  kern<<<cfg->num_envs / V2_E, V2_THREADS, smem, st>>>(*cfg, *buf, *args);
+  kern<<<cfg->num_envs / V2_E, V2_THREADS, smem, st>>>(*cfg, *buf, *args, dev);
   DWBC_LAUNCH_CHECK();
   return DWBC_OK;
 }

@@ -560,10 +560,19 @@ struct LossArgs {
   float clip, c_value, c_ent, c_reg, rho;
   int clipped_value;
   const float* ts_target; const float* ts_pos; const float* ts_vel; const float* ts_coef; float ts_w;      // arm torque supervision (PPO:224-239)
+  const float* sched;                     // optional device (c_reg, rho, ts_w) in place of the three fields (dwbc_ppo_minibatch_grad_sched)
 };
 
 __global__ void __launch_bounds__(128) ppo_loss_kernel(const LossArgs a) {
   __shared__ float red[5 + 32][4];
+  __shared__ float sched_s[3];            // the schedule values, loaded once per CTA
+  if (threadIdx.x == 0) {
+    sched_s[0] = a.sched ? a.sched[0] : a.c_reg;
+    sched_s[1] = a.sched ? a.sched[1] : a.rho;
+    sched_s[2] = a.sched ? a.sched[2] : a.ts_w;
+  }
+  __syncthreads();
+  const float c_reg = sched_s[0], rho = sched_s[1], ts_w = sched_s[2];
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   const bool on = r < a.rows;
   const float inv2m = 1.0f / (2.0f * (float)a.rows), invm = 1.0f / (float)a.rows;
@@ -583,7 +592,7 @@ __global__ void __launch_bounds__(128) ppo_loss_kernel(const LossArgs a) {
       ent[c] += 0.5f + LOG_SQRT_2PI + logf(sg);                                  // AC:326-331 (0.5 log 2pi == log sqrt 2pi)
     }
     const float a0 = a.adv[2 * src], a1 = a.adv[2 * src + 1];
-    const float mix[2] = {a0 + a.rho * a1, a1 + a.rho * a0};                       // PPO:199-201
+    const float mix[2] = {a0 + rho * a1, a1 + rho * a0};                           // PPO:199-201
     float glp[2];
 #pragma unroll
     for (int c = 0; c < 2; ++c) {
@@ -612,7 +621,7 @@ __global__ void __launch_bounds__(128) ppo_loss_kernel(const LossArgs a) {
           const float e = kp * (mu[i] + a.ts_coef[2 * n_arm + j] - a.ts_pos[src * n_arm + j]) - a.ts_coef[n_arm + j] * a.ts_vel[src * n_arm + j] -
                           a.ts_target[src * n_arm + j];
           l_ts += e * e;
-          gmu += 2.0f * a.ts_w / ((float)a.rows * (float)n_arm) * e * kp * (1.0f - mu[i] * mu[i]);
+          gmu += 2.0f * ts_w / ((float)a.rows * (float)n_arm) * e * kp * (1.0f - mu[i] * mu[i]);
         }
         if (c == 0) a.g_leg[(int64_t)r * a.gleg_ld + i] = gmu;
         else a.g_arm[(int64_t)r * a.garm_ld + (i - a.n_leg)] = gmu;
@@ -654,7 +663,7 @@ __global__ void __launch_bounds__(128) ppo_loss_kernel(const LossArgs a) {
     }
     nrm = sqrtf(nrm);
     l_reg = nrm;
-    const float s = nrm > 0.0f ? a.c_reg * invm / nrm : 0.0f;
+    const float s = nrm > 0.0f ? c_reg * invm / nrm : 0.0f;
     for (int i = 0; i < a.latent; ++i)
       a.g_z[(int64_t)r * a.zld + i] = s * (a.zp[(int64_t)r * a.zld + i] - zhr[i]);
   }
@@ -977,8 +986,9 @@ extern "C" int dwbc_hist_latent(const DwbcNetCfg* net, const float* params, cons
   return hist_latent_only(*net, params, obs, nullptr, obs_stride, rows, p, out, ld_out, (cudaStream_t)stream);
 }
 
-extern "C" int dwbc_ppo_minibatch_grad(const DwbcNetCfg* net, const float* params, const DwbcStorage* s, const int64_t* idx, int32_t M,
-                                       const DwbcPpoHyper* hp, float* grad, float* losses_out, void* workspace, dwbc_stream_t stream) {
+// sched: optional device (priv_reg_coef, mixing_ratio, torque_supervision_weight) read by the loss kernels in place of hp's fields
+static int ppo_minibatch_grad(const DwbcNetCfg* net, const float* params, const DwbcStorage* s, const int64_t* idx, int32_t M,
+                              const DwbcPpoHyper* hp, const float* sched, float* grad, float* losses_out, void* workspace, dwbc_stream_t stream) {
   TRY(check_net(net));
   if (!params || !s || !idx || !hp || !grad || !losses_out || !workspace || M <= 0) return DWBC_ERR_ARG;
   if (!s->observations || !s->actions || !s->values || !s->returns || !s->advantages || !s->log_prob) return DWBC_ERR_ARG;
@@ -1013,7 +1023,7 @@ extern "C" int dwbc_ppo_minibatch_grad(const DwbcNetCfg* net, const float* param
     f.clip = hp->clip_param; f.c_value = hp->value_loss_coef; f.c_ent = hp->entropy_coef; f.c_reg = hp->priv_reg_coef; f.rho = hp->mixing_ratio;
     f.clipped_value = hp->use_clipped_value_loss;
     f.ts_target = s->target_arm_torques; f.ts_pos = s->current_arm_dof_pos; f.ts_vel = s->current_arm_dof_vel; f.ts_coef = hp->arm_coefs;
-    f.ts_w = hp->torque_supervision_weight;
+    f.ts_w = hp->torque_supervision_weight; f.sched = sched;
     TRY(launch_pack2(ch.pl, st));
     TRY(launch_chain2(&ch.b[0].pr, &ch.b[1].pr, f, x3, p.queue, st));
     TRY(launch_chain2(&ch.b[2].pr, &ch.b[3].pr, FinArgs{}, x3, p.queue, st, true));      // downwards: the last tiles are still in L2
@@ -1032,7 +1042,7 @@ extern "C" int dwbc_ppo_minibatch_grad(const DwbcNetCfg* net, const float* param
   a.clip = hp->clip_param; a.c_value = hp->value_loss_coef; a.c_ent = hp->entropy_coef; a.c_reg = hp->priv_reg_coef; a.rho = hp->mixing_ratio;
   a.clipped_value = hp->use_clipped_value_loss;
   a.ts_target = s->target_arm_torques; a.ts_pos = s->current_arm_dof_pos; a.ts_vel = s->current_arm_dof_vel; a.ts_coef = hp->arm_coefs;
-  a.ts_w = hp->torque_supervision_weight;
+  a.ts_w = hp->torque_supervision_weight; a.sched = sched;
   ppo_loss_kernel<<<(rows + 127) / 128, 128, 0, st>>>(a);
   DWBC_LAUNCH_CHECK();
 
@@ -1100,6 +1110,18 @@ extern "C" int dwbc_ppo_minibatch_grad(const DwbcNetCfg* net, const float* param
     }
   }
   return DWBC_OK;
+}
+
+extern "C" int dwbc_ppo_minibatch_grad(const DwbcNetCfg* net, const float* params, const DwbcStorage* s, const int64_t* idx, int32_t M,
+                                       const DwbcPpoHyper* hp, float* grad, float* losses_out, void* workspace, dwbc_stream_t stream) {
+  return ppo_minibatch_grad(net, params, s, idx, M, hp, nullptr, grad, losses_out, workspace, stream);
+}
+
+extern "C" int dwbc_ppo_minibatch_grad_sched(const DwbcNetCfg* net, const float* params, const DwbcStorage* s, const int64_t* idx, int32_t M,
+                                             const DwbcPpoHyper* hp, const float* sched, float* grad, float* losses_out, void* workspace,
+                                             dwbc_stream_t stream) {
+  if (!sched) return DWBC_ERR_ARG;
+  return ppo_minibatch_grad(net, params, s, idx, M, hp, sched, grad, losses_out, workspace, stream);
 }
 
 extern "C" int dwbc_dagger_minibatch_grad(const DwbcNetCfg* net, const float* params, const DwbcStorage* s, const int64_t* idx, int32_t M,

@@ -98,6 +98,9 @@ struct FinArgs {
   // ts_coef = [3][n_arm] default p gains, d gains, default dof positions; ts_w = schedule weight (PPO:304-305); losses[4] += mean loss
   const float* ts_target; const float* ts_pos; const float* ts_vel; const float* ts_coef;
   float ts_w;
+  // optional device (c_reg, rho, ts_w) in place of the three fields (dwbc_ppo_minibatch_grad_sched): chain2_kernel loads them once per CTA into
+  // C2Shared, and the hooks take them from there
+  const float* sched;
 };
 
 struct C2Launch {
@@ -156,6 +159,7 @@ __global__ void pack_weights2_kernel(const __grid_constant__ C2PackList pl) {
 struct C2Shared {
   uint64_t w_full, w_free, ld_bar;
   int item, last;
+  float c_reg, rho, ts_w;    // schedule values of the update hooks (FinArgs fields or *FinArgs.sched)
 };
 
 // Slot of the update hooks' warp sums: a worker warp owns 16 rows of a tile, so row m belongs to slot m / 16 = 8 tile + warp.  The last
@@ -312,14 +316,14 @@ __device__ __forceinline__ void c2_fin_act(const FinArgs& f, int c, int64_t m, b
 // PPO:318-323) on act_inference(obs)[:, -n_arm:] (PPO:230: the arm means this hook holds), loss = w * mean((tau - target)^2) (PPO:236-238).
 // Returns (squared error, d loss / d pre-tanh output).  Deliberately NOT inlined and scalar-only (no array leaves the caller's registers): the
 // optional branch must not cost the hot epilogue anything.
-__device__ __noinline__ float2 c2_fin_torque(const FinArgs& f, int64_t src, int cnt, int i, float mu) {
+__device__ __noinline__ float2 c2_fin_torque(const FinArgs& f, int64_t src, int cnt, int i, float mu, float ts_w) {
   const float kp = f.ts_coef[i];
   const float e = kp * (mu + f.ts_coef[2 * cnt + i] - f.ts_pos[src * cnt + i]) - f.ts_coef[cnt + i] * f.ts_vel[src * cnt + i] - f.ts_target[src * cnt + i];
-  return make_float2(e * e, 2.0f * f.ts_w / ((float)f.rows * (float)cnt) * e * kp * (1.0f - mu * mu));
+  return make_float2(e * e, 2.0f * ts_w / ((float)f.rows * (float)cnt) * e * kp * (1.0f - mu * mu));
 }
 // FIN_PPO (AC:341-345, PPO:199-205): log-prob of the stored action, ratio, mixed advantage, clipped surrogate, entropy and
 // the gradients w.r.t. the mean (through the tanh, AC:157,170) and std of this group
-__device__ __forceinline__ void c2_fin_ppo(const FinArgs& f, int c, int64_t m, bool on, const float* v, int lane) {
+__device__ __forceinline__ void c2_fin_ppo(const FinArgs& f, int c, int64_t m, bool on, const float* v, int lane, float rho, float ts_w) {
   const int off = c == 0 ? 0 : f.n_leg, cnt = c == 0 ? f.n_leg : f.n_act - f.n_leg;
   const bool vec2 = ((f.n_act | f.n_leg) & 1) == 0;
   const float inv2m = 1.0f / (2.0f * (float)f.rows);
@@ -341,7 +345,7 @@ __device__ __forceinline__ void c2_fin_ppo(const FinArgs& f, int c, int64_t m, b
         l_ent += 0.5f + C2_LOG_SQRT_2PI + ls;
       }
     }
-    const float mix = c == 0 ? adv.x + f.rho * adv.y : adv.y + f.rho * adv.x;      // PPO:199-201
+    const float mix = c == 0 ? adv.x + rho * adv.y : adv.y + rho * adv.x;          // PPO:199-201
     const float ratio = expf(lp - old_lp);                                           // PPO:202
     const float rc = fminf(fmaxf(ratio, 1.0f - f.clip), 1.0f + f.clip);
     const float s1 = -mix * ratio, s2 = -mix * rc;                                   // PPO:203-205
@@ -364,7 +368,7 @@ __device__ __forceinline__ void c2_fin_ppo(const FinArgs& f, int c, int64_t m, b
     if (c == 1 && f.ts_target != nullptr) {
 #pragma unroll
       for (int i = 0; i < C2_GRP; ++i)
-        if (i < cnt) { const float2 t = c2_fin_torque(f, src, cnt, i, v[i]); l_ts += t.x; gm[i] += t.y; }
+        if (i < cnt) { const float2 t = c2_fin_torque(f, src, cnt, i, v[i], ts_w); l_ts += t.x; gm[i] += t.y; }
     }
     float* grow = c == 0 ? f.g_leg + m * f.gleg_ld : f.g_arm + m * f.garm_ld;
     if ((gld & 3) == 0) {
@@ -425,7 +429,7 @@ __device__ __forceinline__ void c2_fin_value(const FinArgs& f, int c, int64_t m,
   if (lane == 0) c2_fin_slot(f, m)[C2P_VAL + c] = s;
 }
 // FIN_REG (PPO:174-177): || z_priv - sg(z_hist) ||_2 per row, mean over rows
-__device__ __forceinline__ void c2_fin_reg(const FinArgs& f, int64_t m, bool on, const float* v, int lane) {
+__device__ __forceinline__ void c2_fin_reg(const FinArgs& f, int64_t m, bool on, const float* v, int lane, float c_reg) {
   const float invm = 1.0f / (float)f.rows;
   float nrm = 0.0f;
   if (on) {
@@ -435,7 +439,7 @@ __device__ __forceinline__ void c2_fin_reg(const FinArgs& f, int64_t m, bool on,
     for (int i = 0; i < 32; ++i)
       if (i < f.latent) { const float d = v[i] - zhr[i]; nrm += d * d; }
     nrm = sqrtf(nrm);
-    const float s = nrm > 0.0f ? f.c_reg * invm / nrm : 0.0f;
+    const float s = nrm > 0.0f ? c_reg * invm / nrm : 0.0f;
 #pragma unroll
     for (int i = 0; i < 32; ++i)
       if (i < f.gz_ld) f.g_z[m * f.gz_ld + i] = i < f.latent ? s * (v[i] - zhr[i]) : 0.0f;
@@ -539,6 +543,10 @@ __global__ void __launch_bounds__(C2_THREADS, 1) chain2_kernel(const __grid_cons
     tc_mbar_init(&sh.w_free, 1);
     tc_mbar_init(&sh.ld_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    const float* sc = L.fin.sched;
+    sh.c_reg = sc ? sc[0] : L.fin.c_reg;
+    sh.rho = sc ? sc[1] : L.fin.rho;
+    sh.ts_w = sc ? sc[2] : L.fin.ts_w;
   }
   __syncthreads();
   const int n_pair_items = L.np2 * L.nprog;
@@ -798,9 +806,9 @@ __global__ void __launch_bounds__(C2_THREADS, 1) chain2_kernel(const __grid_cons
             if (o.fin != FIN_NONE && u == 0) {               // the head's outputs sit in chunk 0: the lanes holding chunk 1 only take part in the warp sums
               const bool fon = on && hh == 0;
               if (o.fin == FIN_ACT) c2_fin_act(L.fin, o.fin_c, m0 + r, fon, v);
-              else if (o.fin == FIN_PPO) c2_fin_ppo(L.fin, o.fin_c, m0 + r, fon, v, lane);
+              else if (o.fin == FIN_PPO) c2_fin_ppo(L.fin, o.fin_c, m0 + r, fon, v, lane, sh.rho, sh.ts_w);
               else if (o.fin == FIN_VALUE) c2_fin_value(L.fin, o.fin_c, m0 + r, fon, v[0], lane);
-              else c2_fin_reg(L.fin, m0 + r, fon, v, lane);
+              else c2_fin_reg(L.fin, m0 + r, fon, v, lane, sh.c_reg);
             }
             if (active && o.y != nullptr && !o.y_img && on) {       // straight from the registers: 128 contiguous bytes per thread
               float* yr = o.y + (m0 + r) * o.ldy + c0;

@@ -32,6 +32,7 @@ struct AdamArgs {
   const double* sumsq;                   // [nparts] partials of sumsq_kernel
   int nparts;
   float* norm_out;
+  const float* bias_row;                 // optional device (step_size, bc2_sqrt) in place of the two fields (dwbc_clip_adam_step_table)
 };
 
 // Every block sums the partials itself, in the same fixed order (thread t: partials t, t + 256, ...; then a fixed tree)
@@ -52,16 +53,17 @@ __device__ __forceinline__ double sum_partials(const double* __restrict__ part, 
 __global__ void __launch_bounds__(256) clip_adam_kernel(const AdamArgs a) {
   const float total = (float)sqrt(sum_partials(a.sumsq, a.nparts));  // clip_grad_norm_: ||g||_2 over all tensors
   const float coef = fminf(a.max_norm / (total + 1e-6f), 1.0f);
+  const float step_size = a.bias_row ? a.bias_row[0] : a.step_size, bc2_sqrt = a.bias_row ? a.bias_row[1] : a.bc2_sqrt;
   if (a.norm_out && blockIdx.x == 0 && threadIdx.x == 0) *a.norm_out = total;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += (int64_t)gridDim.x * blockDim.x) {
     const float g = (a.g[i] * a.scale) * coef;
     const float m = a.m[i] * a.beta1 + g * (1.0f - a.beta1);
     const float v = a.v[i] * a.beta2 + (g * g) * (1.0f - a.beta2);
-    const float denom = sqrtf(v) / a.bc2_sqrt + a.eps;
+    const float denom = sqrtf(v) / bc2_sqrt + a.eps;
     a.g[i] = g;  // leave the clipped gradient behind (what .grad holds after PPO:245)
     a.m[i] = m;
     a.v[i] = v;
-    a.p[i] = a.p[i] - a.step_size * (m / denom);
+    a.p[i] = a.p[i] - step_size * (m / denom);
   }
 }
 
@@ -74,9 +76,22 @@ __global__ void min_std_kernel(float* __restrict__ std, const float* __restrict_
 
 using namespace dwbc;
 
-extern "C" int dwbc_clip_adam_step(float* params, float* grad, float* adam_m, float* adam_v, int64_t first, int64_t count,
-                                   const DwbcPpoHyper* hp, int32_t step, double* norm_scratch, float* grad_norm_out,
-                                   dwbc_stream_t stream) {
+// Adam's bias correction of 1-based step `step` as the host computes it: (lr / (1 - beta1^step), sqrt(1 - beta2^step)), double, then float
+static void adam_bias_row(const DwbcPpoHyper* hp, int32_t step, float* row) {
+  const double bc1 = 1.0 - pow((double)hp->beta1, (double)step), bc2 = 1.0 - pow((double)hp->beta2, (double)step);
+  row[0] = (float)((double)hp->lr / bc1);
+  row[1] = (float)sqrt(bc2);
+}
+
+extern "C" int dwbc_adam_bias_correction(const DwbcPpoHyper* hp, int32_t first_step, int32_t n, float* out) {
+  if (!hp || !out || first_step < 1 || n < 0) return DWBC_ERR_ARG;
+  for (int32_t i = 0; i < n; ++i) adam_bias_row(hp, first_step + i, out + 2 * i);
+  return DWBC_OK;
+}
+
+// adam_table: optional device rows (lr / bc1, sqrt(bc2)), row step - 1 read by the kernel in place of the host computation
+static int clip_adam_step(float* params, float* grad, float* adam_m, float* adam_v, int64_t first, int64_t count, const DwbcPpoHyper* hp,
+                          int32_t step, const float* adam_table, double* norm_scratch, float* grad_norm_out, dwbc_stream_t stream) {
   if (!params || !grad || !adam_m || !adam_v || !hp || !norm_scratch || count <= 0 || first < 0 || step < 1) return DWBC_ERR_ARG;
   cudaStream_t st = (cudaStream_t)stream;
   const float scale = hp->grad_scale == 0.0f ? 1.0f : hp->grad_scale;
@@ -85,12 +100,26 @@ extern "C" int dwbc_clip_adam_step(float* params, float* grad, float* adam_m, fl
   if (grid < 1) grid = 1;
   sumsq_kernel<<<grid, 256, 0, st>>>(grad + first, count, scale, norm_scratch);
   DWBC_LAUNCH_CHECK();
-  const double bc1 = 1.0 - pow((double)hp->beta1, (double)step), bc2 = 1.0 - pow((double)hp->beta2, (double)step);
+  float row[2] = {0.0f, 0.0f};
+  if (!adam_table) adam_bias_row(hp, step, row);
   AdamArgs a{params + first, grad + first, adam_m + first, adam_v + first, count, scale, hp->max_grad_norm, hp->beta1, hp->beta2,
-             hp->adam_eps, (float)((double)hp->lr / bc1), (float)sqrt(bc2), norm_scratch, grid, grad_norm_out};
+             hp->adam_eps, row[0], row[1], norm_scratch, grid, grad_norm_out, adam_table ? adam_table + 2 * (int64_t)(step - 1) : nullptr};
   clip_adam_kernel<<<grid, 256, 0, st>>>(a);
   DWBC_LAUNCH_CHECK();
   return DWBC_OK;
+}
+
+extern "C" int dwbc_clip_adam_step(float* params, float* grad, float* adam_m, float* adam_v, int64_t first, int64_t count,
+                                   const DwbcPpoHyper* hp, int32_t step, double* norm_scratch, float* grad_norm_out,
+                                   dwbc_stream_t stream) {
+  return clip_adam_step(params, grad, adam_m, adam_v, first, count, hp, step, nullptr, norm_scratch, grad_norm_out, stream);
+}
+
+extern "C" int dwbc_clip_adam_step_table(float* params, float* grad, float* adam_m, float* adam_v, int64_t first, int64_t count,
+                                         const DwbcPpoHyper* hp, int32_t step, const float* adam_table, double* norm_scratch,
+                                         float* grad_norm_out, dwbc_stream_t stream) {
+  if (!adam_table) return DWBC_ERR_ARG;
+  return clip_adam_step(params, grad, adam_m, adam_v, first, count, hp, step, adam_table, norm_scratch, grad_norm_out, stream);
 }
 
 extern "C" int dwbc_enforce_min_std(float* params, int64_t off_std, const float* min_std, int32_t n, dwbc_stream_t stream) {
@@ -103,7 +132,9 @@ extern "C" int dwbc_enforce_min_std(float* params, int64_t off_std, const float*
 unsigned long long dwbc_launch_counter = 0;
 extern "C" uint64_t dwbc_launch_count(void) { return dwbc_launch_counter; }
 
-extern "C" const char* dwbc_version(void) { return "dwbc-b200 0.1 (sm_90a, abi 3)"; }
+extern "C" const char* dwbc_version(void) { return "dwbc-b200 0.1 (sm_90a, abi 5)"; }
+
+extern "C" int64_t dwbc_step_device_size(void) { return sizeof(DwbcStepDevice); }
 
 extern "C" void dwbc_struct_sizes(int64_t out[6]) {
   out[0] = sizeof(DwbcEnvCfg); out[1] = sizeof(DwbcEnvBuffers); out[2] = sizeof(DwbcStepArgs);

@@ -163,6 +163,7 @@ class FusedWidowGo1Core:
         self._cfg = make_env_cfg(p, self._sums_stride)
         self._buf = L.EnvBuffers()
         self._args = L.StepArgs()
+        self._dev_step = None          # device DwbcStepDevice of a captured rollout (set_device_step)
         # True: always the warp-per-env kernel, which also runs by itself when N is not a multiple of 32 or a state row block is not
         # 16-byte aligned (the observation target and the history must be 16-byte aligned for both kernels)
         self._args.generic_kernel = int(generic_kernel)
@@ -383,12 +384,34 @@ class FusedWidowGo1Core:
         self.reset_count = None
         if self.sync_stats:
             self._stats.zero_()        # per-step episode statistics (WG:743-750); without them the accumulators are read by episode_stats()
-        L.check(self._lib.dwbc_post_physics_step(C.addressof(self._cfg), C.addressof(self._buf), C.addressof(a), L.stream_ptr()),
-                "dwbc_post_physics_step")
+        if self._dev_step is None:
+            L.check(self._lib.dwbc_post_physics_step(C.addressof(self._cfg), C.addressof(self._buf), C.addressof(a), L.stream_ptr()),
+                    "dwbc_post_physics_step")
+        else:
+            L.check(self._lib.dwbc_post_physics_step_device(C.addressof(self._cfg), C.addressof(self._buf), C.addressof(a),
+                                                            L.ptr(self._dev_step, torch.uint8), L.stream_ptr()), "dwbc_post_physics_step_device")
         self.extras["time_outs"] = self.time_out_buf
         self.extras["dwbc_stored_rows"] = getattr(self, "_stored_rows", None)
         if self.sync_stats:
             self._fill_episode_extras()
+
+    def step_record(self) -> torch.Tensor:
+        """The DwbcStepDevice of the next post_physics_step (uint8 host tensor): the step, the push interval and the curriculum values
+        this core would pass by value.  Copied to the device record given to `set_device_step`, it lets a captured post_physics_step
+        read them at run time; each call then advances the step on the device."""
+        r, a = L.StepDevice(), self._args
+        r.step = self.common_step_counter + 1
+        r.push_interval = int(self.p.push_interval) if self.p.push_robots else 0
+        first, end = L.StepArgs.lin_vel_x.offset, L.StepArgs.generic_kernel.offset
+        C.memmove(C.addressof(r) + L.StepDevice.lin_vel_x.offset, C.addressof(a) + first, end - first)
+        return torch.frombuffer(bytearray(bytes(r)), dtype=torch.uint8)
+
+    def set_device_step(self, record: Optional[torch.Tensor]):
+        """Make post_physics_step launch through dwbc_post_physics_step_device with this device DwbcStepDevice ([sizeof] uint8 CUDA
+        tensor) or, with None, through dwbc_post_physics_step with the host fields again."""
+        if record is not None and (record.dtype != torch.uint8 or record.numel() != C.sizeof(L.StepDevice)):
+            raise L.DwbcError(f"the device step record is a uint8 tensor of {C.sizeof(L.StepDevice)} bytes")
+        self._dev_step = record
 
     def episode_stats(self, reset: bool = True):
         """`extras['episode']` over every episode that ended since the last call (one D2H read; for sync_stats=False loops that log once per

@@ -22,6 +22,7 @@ import torch
 from . import _lib as L
 from . import shard
 from .actor_critic import FlatActorCritic
+from .graphs import HostUpload
 from .storage import FusedRolloutStorage
 
 
@@ -58,7 +59,7 @@ class FusedPPO:
                  use_clipped_value_loss=True, schedule="fixed", desired_kl=0.01, device="cuda:0",
                  mixing_schedule=(0.5, 2000, 4000), torque_supervision=False, torque_supervision_schedule=(0.1, 1000, 1000),
                  adaptive_arm_gains=False, min_policy_std=None, dagger_update_freq=20, priv_reg_coef_schedual=(0, 0, 0, 1),
-                 world_size=1, process_group=None, precision="tf32x3"):
+                 world_size=1, process_group=None, precision="tf32x3", cuda_graphs=False):
         if adaptive_arm_gains:
             raise L.DwbcError("adaptive_arm_gains (a 12-output arm head, AC:111-125,214-215; off for widowGo1, WGC:168) is not implemented")
         if schedule != "fixed":
@@ -98,6 +99,12 @@ class FusedPPO:
         self.transition = FusedRolloutStorage.Transition()
         self._eps = None
         self.generator = None
+        # cuda_graphs: update() and update_dagger() run as CUDA graphs captured on their first call for a key (graph_key) and replayed
+        # afterwards, with the same bits as the eager calls (DESIGN §11)
+        if cuda_graphs and world_size > 1:
+            raise L.DwbcError("cuda_graphs=True does not capture the multi-GPU all-reduce: use world_size == 1")
+        self.cuda_graphs = bool(cuda_graphs)
+        self._graphs = {}
 
     # ------------------------------------------------------------------ plumbing
     def init_storage(self, num_envs, num_transitions_per_env, actor_obs_shape, critic_obs_shape, action_shape):
@@ -275,6 +282,8 @@ class FusedPPO:
 
     # ------------------------------------------------------------------ update (PPO:152-263)
     def update(self, indices=None, on_step=None):
+        if self.cuda_graphs and on_step is None:
+            return self._update_graphed("ppo", indices)
         ac, s, hp = self.actor_critic, self.storage, self._fill_hp()
         self._set_precision()
         self._packed = False                      # the parameters move (and the workspace is re-used with another row count)
@@ -283,37 +292,65 @@ class FusedPPO:
         indices = indices.to(torch.int64).contiguous()
         mbs = indices.numel() // self.num_mini_batches
         ws = self._workspace(mbs)
+        self._ppo_launches(hp, indices, mbs, ws, on_step)
+        return self._ppo_finish(hp)
+
+    def _zh_buffer(self):
+        s = self.storage
+        total = s.num_envs * s.num_transitions_per_env
+        lld = (self.actor_critic.priv_dims[-1] + 3) // 4 * 4
+        if self._zh_all is None or self._zh_all.shape[0] != total:
+            self._zh_all = torch.zeros(total, lld, device=self.device)
+        return self._zh_all
+
+    def _ppo_launches(self, hp, indices, mbs, ws, on_step=None, dev=None):
+        """Every launch of one update().  dev = (sched, adam_table) device pointers when capturing: the schedule values and the Adam
+        bias correction are then read at run time (row k of the table for mini-batch k), and optimizer.step is left to the caller."""
+        ac, s = self.actor_critic, self.storage
         self._losses.zero_()
         k = 0
         # The regulariser target z_hist (PPO:175-176) is detached, so update() never moves the history encoder (zero gradient ->
         # zero Adam step): evaluate it once per storage row instead of once per (epoch, row).
         total = s.num_envs * s.num_transitions_per_env
-        lld = (ac.priv_dims[-1] + 3) // 4 * 4
-        if self._zh_all is None or self._zh_all.shape[0] != total:
-            self._zh_all = torch.zeros(total, lld, device=self.device)
+        zh = self._zh_buffer()
+        lld = zh.shape[1]
         obs_flat = s.observations.view(total, -1)
         for r0 in range(0, total, mbs):
             nrow = min(mbs, total - r0)
             L.check(self._lib.dwbc_hist_latent(C.addressof(ac.net_cfg), L.ptr(ac.flat), L.ptr(obs_flat[r0:]), obs_flat.stride(0),
-                                               L.ptr(self._zh_all[r0:]), lld, nrow, L.ptr(ws), L.stream_ptr()), "dwbc_hist_latent")
-        s.set_hist_latent(self._zh_all)
+                                               L.ptr(zh[r0:]), lld, nrow, L.ptr(ws), L.stream_ptr()), "dwbc_hist_latent")
+        s.set_hist_latent(zh)
         for batch_idx in s.mini_batch_generator(self.num_mini_batches, self.num_learning_epochs, indices):
-            L.check(self._lib.dwbc_ppo_minibatch_grad(C.addressof(ac.net_cfg), L.ptr(ac.flat), s.c_struct_ptr(), L.ptr(batch_idx), mbs,
-                                                      C.addressof(hp), L.ptr(self.grad), L.ptr(self._losses), L.ptr(ws), L.stream_ptr()),
-                    "dwbc_ppo_minibatch_grad")
+            if dev is None:
+                L.check(self._lib.dwbc_ppo_minibatch_grad(C.addressof(ac.net_cfg), L.ptr(ac.flat), s.c_struct_ptr(), L.ptr(batch_idx), mbs,
+                                                          C.addressof(hp), L.ptr(self.grad), L.ptr(self._losses), L.ptr(ws), L.stream_ptr()),
+                        "dwbc_ppo_minibatch_grad")
+            else:
+                L.check(self._lib.dwbc_ppo_minibatch_grad_sched(C.addressof(ac.net_cfg), L.ptr(ac.flat), s.c_struct_ptr(), L.ptr(batch_idx),
+                                                                mbs, C.addressof(hp), dev[0], L.ptr(self.grad), L.ptr(self._losses), L.ptr(ws),
+                                                                L.stream_ptr()), "dwbc_ppo_minibatch_grad_sched")
             self._allreduce(0, ac.num_params)
             if on_step is not None:
                 on_step(k, "grad")
-            self.optimizer.step += 1
-            L.check(self._lib.dwbc_clip_adam_step(L.ptr(ac.flat), L.ptr(self.grad), L.ptr(self.optimizer.m), L.ptr(self.optimizer.v), 0,
-                                                  ac.num_params, C.addressof(hp), self.optimizer.step, L.ptr(self._norm_scratch),
-                                                  L.ptr(self._grad_norm), L.stream_ptr()), "dwbc_clip_adam_step")
+            opt = self.optimizer
+            if dev is None:
+                opt.step += 1
+                L.check(self._lib.dwbc_clip_adam_step(L.ptr(ac.flat), L.ptr(self.grad), L.ptr(opt.m), L.ptr(opt.v), 0, ac.num_params,
+                                                      C.addressof(hp), opt.step, L.ptr(self._norm_scratch), L.ptr(self._grad_norm),
+                                                      L.stream_ptr()), "dwbc_clip_adam_step")
+            else:
+                L.check(self._lib.dwbc_clip_adam_step_table(L.ptr(ac.flat), L.ptr(self.grad), L.ptr(opt.m), L.ptr(opt.v), 0, ac.num_params,
+                                                            C.addressof(hp), k + 1, dev[1], L.ptr(self._norm_scratch), L.ptr(self._grad_norm),
+                                                            L.stream_ptr()), "dwbc_clip_adam_step_table")
             if on_step is not None:
                 on_step(k, "step")
             k += 1
+        s.set_hist_latent(None)
+
+    def _ppo_finish(self, hp):
+        s = self.storage
         num_updates = self.num_learning_epochs * self.num_mini_batches
         losses = (self._losses / num_updates).tolist()                                   # single sync per update
-        s.set_hist_latent(None)
         s.clear()
         value_mixing_ratio, priv_reg_coef = hp.mixing_ratio, hp.priv_reg_coef
         self.counter += 1                                                                 # PPO:259
@@ -324,7 +361,9 @@ class FusedPPO:
 
     def update_dagger(self, indices=None):
         """PPO:265-291."""
-        ac, s, hp = self.actor_critic, self.storage, self._fill_hp()
+        if self.cuda_graphs:
+            return self._update_graphed("dagger", indices)
+        s, hp = self.storage, self._fill_hp()
         self._set_precision()
         self._packed = False
         if indices is None:
@@ -332,22 +371,95 @@ class FusedPPO:
         indices = indices.to(torch.int64).contiguous()
         mbs = indices.numel() // self.num_mini_batches
         ws = self._workspace(mbs)
+        self._dagger_launches(hp, indices, mbs, ws)
+        return self._dagger_finish()
+
+    def _dagger_launches(self, hp, indices, mbs, ws, dev=None):
+        """Every launch of one update_dagger(); dev as in _ppo_launches (only its Adam table is read)."""
+        ac, s = self.actor_critic, self.storage
         self._losses.zero_()
         hf, hc = ac.hist_range
         opt = self.hist_encoder_optimizer
-        for batch_idx in s.mini_batch_generator(self.num_mini_batches, self.num_learning_epochs, indices):
+        for k, batch_idx in enumerate(s.mini_batch_generator(self.num_mini_batches, self.num_learning_epochs, indices)):
             L.check(self._lib.dwbc_dagger_minibatch_grad(C.addressof(ac.net_cfg), L.ptr(ac.flat), s.c_struct_ptr(), L.ptr(batch_idx), mbs,
                                                          L.ptr(self.grad), L.ptr(self._losses), L.ptr(ws), L.stream_ptr()),
                     "dwbc_dagger_minibatch_grad")
             self._allreduce(hf, hc)
-            opt.step += 1
-            L.check(self._lib.dwbc_clip_adam_step(L.ptr(ac.flat), L.ptr(self.grad), L.ptr(opt.m), L.ptr(opt.v), hf, hc, C.addressof(hp),
-                                                  opt.step, L.ptr(self._norm_scratch), None, L.stream_ptr()), "dwbc_clip_adam_step")
+            if dev is None:
+                opt.step += 1
+                L.check(self._lib.dwbc_clip_adam_step(L.ptr(ac.flat), L.ptr(self.grad), L.ptr(opt.m), L.ptr(opt.v), hf, hc, C.addressof(hp),
+                                                      opt.step, L.ptr(self._norm_scratch), None, L.stream_ptr()), "dwbc_clip_adam_step")
+            else:
+                L.check(self._lib.dwbc_clip_adam_step_table(L.ptr(ac.flat), L.ptr(self.grad), L.ptr(opt.m), L.ptr(opt.v), hf, hc,
+                                                            C.addressof(hp), k + 1, dev[1], L.ptr(self._norm_scratch), None, L.stream_ptr()),
+                        "dwbc_clip_adam_step_table")
+
+    def _dagger_finish(self):
         num_updates = self.num_learning_epochs * self.num_mini_batches
         loss = float(self._losses[0]) / num_updates
-        s.clear()
+        self.storage.clear()
         self.counter += 1
         return loss
+
+    # ------------------------------------------------------------------ CUDA graphs of update() / update_dagger()
+    def graph_key(self, kind):
+        """What a captured update depends on beyond the per-iteration scalars: a change re-captures.  Storage shape and buffers,
+        mini-batching, precision, network and workspace, torque supervision, and the hyper-parameters the launches carry by value."""
+        s, ac, h = self.storage, self.actor_critic, self._hp
+        return (kind, s.num_transitions_per_env, s.num_envs, s._obs_all.data_ptr(), self.num_mini_batches, self.num_learning_epochs,
+                self._precision, ac.flat.data_ptr(), bytes(ac.net_cfg), self._ws.data_ptr(), self._ws_rows, self.torque_supervision,
+                h.clip_param, h.value_loss_coef, h.entropy_coef, h.use_clipped_value_loss, h.max_grad_norm, h.lr, h.beta1, h.beta2,
+                h.adam_eps, h.grad_scale, h.arm_coefs)
+
+    def _update_graphed(self, kind, indices):
+        """update() / update_dagger() as one CUDA graph: captured on the first call for a key (graph_key), replayed on later calls.  The
+        permutation is drawn eagerly (same generator call as the eager path) into a fixed buffer; the schedule values and the Adam bias
+        correction of this call's steps travel to the device in one asynchronous stream-ordered copy before the replay."""
+        if self.world_size > 1:
+            raise L.DwbcError("cuda_graphs=True does not capture the multi-GPU all-reduce: use world_size == 1")
+        s, hp = self.storage, self._fill_hp()
+        self._set_precision()
+        self._packed = False
+        if indices is None:
+            indices, _ = s.draw_indices(self.num_mini_batches, self.generator)
+        indices = indices.to(torch.int64).contiguous()
+        mbs = indices.numel() // self.num_mini_batches
+        self._workspace(mbs)
+        if kind == "ppo":
+            self._zh_buffer()
+        n_steps = self.num_learning_epochs * self.num_mini_batches
+        key = self.graph_key(kind) + (indices.numel(),)
+        g = self._graphs.get(kind)
+        if g is None or g["key"] != key:
+            g = self._capture(kind, key, mbs, indices.numel(), n_steps)
+        g["idx"].copy_(indices)
+        opt = self.optimizer if kind == "ppo" else self.hist_encoder_optimizer
+        host = torch.empty(4 + 2 * n_steps, dtype=torch.float32)
+        host[:3] = torch.tensor([hp.priv_reg_coef, hp.mixing_ratio, hp.torque_supervision_weight], dtype=torch.float32)
+        host[3] = 0.0
+        host[4:] = torch.from_numpy(L.adam_bias_correction(hp, opt.step + 1, n_steps).reshape(-1))
+        g["upload"](g["scalars"], host)
+        g["graph"].replay()
+        opt.step += n_steps
+        return self._ppo_finish(hp) if kind == "ppo" else self._dagger_finish()
+
+    def _capture(self, kind, key, mbs, n_idx, n_steps):
+        self._graphs.pop(kind, None)
+        scalars = torch.zeros(4 + 2 * n_steps, device=self.device)          # sched [3], pad, Adam table [n_steps, 2]
+        idx = torch.zeros(n_idx, dtype=torch.int64, device=self.device)
+        hp = L.PpoHyper()
+        C.memmove(C.addressof(hp), C.addressof(self._hp), C.sizeof(hp))
+        dev = (scalars.data_ptr(), scalars.data_ptr() + 16)
+        graph = torch.cuda.CUDAGraph()
+        torch.cuda.synchronize(self.device)
+        with torch.cuda.graph(graph):
+            if kind == "ppo":
+                self._ppo_launches(hp, idx, mbs, self._ws, dev=dev)
+            else:
+                self._dagger_launches(hp, idx, mbs, self._ws, dev=dev)
+        g = dict(key=key, graph=graph, scalars=scalars, idx=idx, hp=hp, upload=HostUpload())
+        self._graphs[kind] = g
+        return g
 
     def enforce_min_std(self):
         if self.min_policy_std is None:

@@ -14,6 +14,10 @@
  * global state (except a launch counter and the clock-stamp pointer of dwbc_debug_set_tc_cycle_buffer), never synchronises and never throws: every function enqueues its kernels on
  * the given stream and returns DWBC_OK or a negative error code.  Structs are passed by
  * pointer to HOST memory and are read before the call returns.
+ *
+ * Every entry point can be captured into a CUDA graph (cudaStreamBeginCapture on `stream`): none synchronises, allocates or queries the
+ * device in a way capture forbids.  A captured launch keeps the by-value parameters of capture time; the values that change between two
+ * replays of a training iteration can instead be read from device memory by the *_device / *_sched / *_table entry points.
  */
 #ifndef DWBC_H
 #define DWBC_H
@@ -194,6 +198,17 @@ typedef struct DwbcStepArgs {
   int32_t reserved_;
 } DwbcStepArgs;
 
+/* Device-resident per-step values of dwbc_post_physics_step_device (CUDA-graph replay).  The caller fills the record with one
+ * stream-ordered copy; its values equal what the host would put into DwbcStepArgs for the same step. */
+typedef struct DwbcStepDevice {
+  uint64_t step;                 /* common_step_counter of the NEXT call (the Philox key); the call adds 1 after using it */
+  int32_t push_interval;         /* do_push = push_interval > 0 && step % push_interval == 0 (WG:934); 0: never push */
+  int32_t reserved_;
+  float lin_vel_x[2], ang_vel_yaw[2], goal_l[2], goal_p[2], goal_y[2]; /* as in DwbcStepArgs */
+  float leg_scale[DWBC_MAX_TERMS], arm_scale[DWBC_MAX_TERMS];
+  float leg_termination_scale, arm_termination_scale;
+} DwbcStepDevice;
+
 /* Replaces WidowGo1.post_physics_step after its four gym.refresh_* calls (WG:875-910),
  * including update_curr_ee_goal (WG:1344-1350), _post_physics_step_callback (WG:917-935),
  * check_termination (WG:937-963), compute_reward (WG:170-205), reset_idx (WG:695-754),
@@ -201,6 +216,13 @@ typedef struct DwbcStepArgs {
  * cfg.measure_heights, LeggedRobot._get_heights (LR:793-829).  One kernel launch. */
 int dwbc_post_physics_step(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, const DwbcStepArgs* args,
                            dwbc_stream_t stream);
+
+/* dwbc_post_physics_step whose step, push decision and curriculum values come from the DEVICE record `device` at run time, so that a
+ * captured launch stays right on every replay (seed, rand_uniform and generic_kernel stay the host fields of `args`; its step, do_push
+ * and curriculum fields are ignored).  The call advances device->step by one in stream order after the kernel has used it.  Only the
+ * 16-envs-per-CTA kernel reads a device record: a call that would take the warp-per-env kernel returns DWBC_ERR_UNSUPPORTED. */
+int dwbc_post_physics_step_device(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, const DwbcStepArgs* args, DwbcStepDevice* device,
+                                  dwbc_stream_t stream);
 
 /* Materialises the uniform table the in-kernel Philox stream would produce:
  * out[N,DWBC_RAND_COLS] (so table mode and Philox mode can be checked against each other). */
@@ -364,6 +386,11 @@ typedef struct DwbcStorage {
 int dwbc_ppo_minibatch_grad(const DwbcNetCfg* net, const float* params, const DwbcStorage* st, const int64_t* idx,
                             int32_t M, const DwbcPpoHyper* hp, float* grad, float* losses_out, void* workspace,
                             dwbc_stream_t stream);
+/* The same, with priv_reg_coef, mixing_ratio and torque_supervision_weight read at run time from the DEVICE array sched[3] instead of
+ * hp's fields (CUDA-graph replay: the schedules move between replays).  Whether the torque branch is on still follows hp and the storage. */
+int dwbc_ppo_minibatch_grad_sched(const DwbcNetCfg* net, const float* params, const DwbcStorage* st, const int64_t* idx,
+                                  int32_t M, const DwbcPpoHyper* hp, const float* sched, float* grad, float* losses_out, void* workspace,
+                                  dwbc_stream_t stream);
 
 /* PPO.update_dagger mini-batch (PPO:273-283): grad of mean ||sg(z_priv) - z_hist||_2 w.r.t. the
  * history-encoder parameters only (other entries of grad are zeroed). losses_out[0] += loss. */
@@ -379,6 +406,16 @@ int dwbc_dagger_minibatch_grad(const DwbcNetCfg* net, const float* params, const
 int dwbc_clip_adam_step(float* params, float* grad, float* adam_m, float* adam_v, int64_t first, int64_t count,
                         const DwbcPpoHyper* hp, int32_t step, double* norm_scratch, float* grad_norm_out,
                         dwbc_stream_t stream);
+/* The same, with Adam's bias correction (lr / bc1, sqrt(bc2)) read at run time from row step - 1 of the DEVICE table adam_table[2 n]
+ * instead of being computed on the host from `step` (CUDA-graph replay).  dwbc_adam_bias_correction fills such rows with exactly the
+ * floats of the host path. */
+int dwbc_clip_adam_step_table(float* params, float* grad, float* adam_m, float* adam_v, int64_t first, int64_t count,
+                              const DwbcPpoHyper* hp, int32_t step, const float* adam_table, double* norm_scratch, float* grad_norm_out,
+                              dwbc_stream_t stream);
+
+/* The (lr / bc1, sqrt(bc2)) rows dwbc_clip_adam_step computes on the host for Adam steps first_step .. first_step + n - 1 (1-based),
+ * written to out[2 * n] in HOST memory: bc = 1 - beta^step in double (glibc pow), lr / bc1 and sqrt(bc2) rounded to float. */
+int dwbc_adam_bias_correction(const DwbcPpoHyper* hp, int32_t first_step, int32_t n, float* out);
 
 /* PPO.enforce_min_std (PPO:293-296): std = max(std, min_std). */
 int dwbc_enforce_min_std(float* params, int64_t off_std, const float* min_std, int32_t n, dwbc_stream_t stream);
@@ -389,6 +426,8 @@ uint64_t dwbc_launch_count(void);
 /* sizeof(DwbcEnvCfg, DwbcEnvBuffers, DwbcStepArgs, DwbcNetCfg, DwbcPpoHyper, DwbcStorage): lets a
  * foreign-language binding verify its struct mirrors at load time. */
 void dwbc_struct_sizes(int64_t out[6]);
+/* sizeof(DwbcStepDevice) */
+int64_t dwbc_step_device_size(void);
 
 #ifdef __cplusplus
 }
