@@ -69,15 +69,6 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 ctr, uint2 key) {
 // uniform in [0,1) with a 24-bit mantissa, like torch.rand(float32)
 __device__ __forceinline__ float u01(uint32_t x) { return (float)(x >> 8) * 5.9604644775390625e-08f; }
 
-// The uniform stream of one env step: value(env, col) = philox(ctr=(env, col/4, step_lo, step_hi), key=seed)[col%4]
-__device__ __forceinline__ float philox_uniform(uint64_t seed, uint64_t step, int env, int col) {
-  uint4 r = philox4x32_10(make_uint4((uint32_t)env, (uint32_t)(col >> 2), (uint32_t)step, (uint32_t)(step >> 32)),
-                          make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
-  int k = col & 3;
-  uint32_t x = k == 0 ? r.x : (k == 1 ? r.y : (k == 2 ? r.z : r.w));
-  return u01(x);
-}
-
 // Fixed-order sums across blocks: every block writes its partials to a slot of its own, then calls this.  It returns true, in every
 // thread, in the block that arrives last (counted on `ticket`, which that block returns to zero for the next launch); that block sees
 // every partial and adds them up in slot order, so the result does not depend on which block ran when.

@@ -71,26 +71,4 @@ __device__ __forceinline__ float4 clip4(float4 v, float c) {
   return make_float4(clipf(v.x, -c, c), clipf(v.y, -c, c), clipf(v.z, -c, c), clipf(v.w, -c, c));
 }
 
-struct Rng {
-  const float* table;
-  uint64_t seed, step;
-  int env;
-  __device__ __forceinline__ float operator()(int col) const {
-    return table ? __ldg(table + (size_t)env * DWBC_RAND_COLS + col) : philox_uniform(seed, step, env, col);
-  }
-};
-
-
-// WG:1337-1342
-static __device__ __noinline__ bool goal_collides(const DwbcEnvCfg& cfg, V3 start, V3 goal) {
-  bool hit = false;
-  for (int s = 0; s < cfg.n_collision_samples; ++s) {
-    V3 p = sphere2cart(lerp3(start, goal, cfg.collision_t[s]));
-    bool inside = (p.x < cfg.collision_upper[0] && p.y < cfg.collision_upper[1] && p.z < cfg.collision_upper[2]) &&
-                  (p.x > cfg.collision_lower[0] && p.y > cfg.collision_lower[1] && p.z > cfg.collision_lower[2]);
-    hit = hit || inside || (p.z < cfg.underground_limit);
-  }
-  return hit;
-}
-
 }  // namespace dwbc

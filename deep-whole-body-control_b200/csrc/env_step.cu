@@ -1,271 +1,43 @@
-// Fused widowGo1 post-physics step: ONE kernel launch per sim step (K1 + K2 of SURVEY.md).
+// Fused widowGo1 post-physics step, warp-per-env kernel: ONE kernel launch per sim step (K1 + K2 of SURVEY.md).
 //
 // Replaces the ~200 ATen launches of WidowGo1.post_physics_step (WG:875-910): derived base
 // state, EE-goal generator, command resampling, push, height scan, termination, the reward-term
 // stack for both channels, episode sums, reset, observation assembly, history shift, obs clip.
 //
-// Mapping: one WARP per environment, 4 warps per CTA.  Every env is independent (SURVEY 3.3),
-// so all control flow is warp-uniform.  Lane d owns DOF d / obs column groups; the handful of
-// scalar quantities (quaternion algebra, goal interpolation, termination) are computed
-// redundantly by all lanes from a shared-memory staging block that was filled with coalesced
-// loads.  The 3 KB history row is read once as 128-bit streaming loads issued before anything
+// Mapping: one WARP per environment, 4 warps per CTA, any shape and shard size.  The TMA kernel
+// (env_step_v2.cu) runs the widowGo1 shapes with 10-step histories on shards that are a multiple of 32;
+// this kernel runs everything else.  Both call the per-env functions of env_step_common.cuh on the
+// env's rows staged in shared memory: this kernel runs the warp functions with its warp and
+// scalar_step() on lane 0.  The history row is read as 128-bit streaming loads issued before anything
 // else (so ~86 KB are in flight per SM), re-emitted into obs_buf and shifted in place.
 //
-// HBM-bound: algorithmic bytes 10 653 B / env-step (SURVEY 8d) -> 6.6 us @ 4096 envs at the
-// measured 6.57 TB/s.  Compiled with -fmad=false so that discrete decisions (collision
-// rejection, command dead-band, termination thresholds) see the same fp32 roundings as the
-// reference's unfused torch arithmetic.
+// Compiled with -fmad=false so that discrete decisions (collision rejection, command dead-band,
+// termination thresholds) see the same fp32 roundings as the reference's unfused torch arithmetic.
 #include <stdlib.h>
 
-#include "env_math.cuh"
+#include "env_step_common.cuh"
 
 namespace dwbc {
 
 constexpr int ENV_WARPS = 4;
 constexpr int MAX_H4 = 8;  // history row <= 8*32 float4 = 1024 floats in registers; longer rows take the streaming form (kLong)
 
-// shared-memory staging block of one warp (float offsets)
+// shared-memory staging block of one warp (float offsets; S_PRIV and S_PROP 16-byte aligned for the float4 write-out)
 enum {
-  S_ROOT = 0, S_DOF = 16, S_EE = 64, S_FS = 80, S_TQ = 104, S_ACT = 128, S_AH = 152, S_GS = 176, S_DS = 204,
-  S_SUM = 276, S_PRIV = 340, S_PROP = 372, S_CF = 468, S_TOTAL = 532
+  S_ROOT = 0, S_DOF = 28, S_EE = 76, S_FS = 84, S_TQ = 108, S_ACT = 132, S_AH = 156, S_GS = 348, S_DS = 376, S_SUM = 448,
+  S_PRIV = 512, S_PROP = 544, S_CF = 640, S_MASS = 700, S_FRIC = 705, S_MOTOR = 708, S_FEAT = 732, S_RP = 748, S_REW = 752, S_TOTAL = 756
 };
-
-// WG:1316-1332 for one env; gs = staged goal_state row (all lanes compute, lane 0 commits)
-__device__ void resample_goal(const DwbcEnvCfg& cfg, const DwbcStepArgs& A, const Rng& rng, float* gs, float yaw,
-                              int col_orn, int col_sph, int lane) {
-  float d[3], o[3];
-  const float ye[3] = {0.0f, 0.0f, yaw};
-#pragma unroll
-  for (int i = 0; i < 3; ++i) {
-    d[i] = cfg.delta_orn_span[i] * rng(col_orn + i) + cfg.delta_orn_lo[i];
-    o[i] = wrap_pi(d[i] + ye[i]);
-  }
-  V3 start = mk(gs[DWBC_GS_GOAL_SPH], gs[DWBC_GS_GOAL_SPH + 1], gs[DWBC_GS_GOAL_SPH + 2]);
-  V3 goal = start;
-  for (int k = 0; k < cfg.max_goal_tries; ++k) {
-    goal = mk(A.goal_l[1] * rng(col_sph + 3 * k) + A.goal_l[0], A.goal_p[1] * rng(col_sph + 3 * k + 1) + A.goal_p[0],
-              A.goal_y[1] * rng(col_sph + 3 * k + 2) + A.goal_y[0]);
-    if (!goal_collides(cfg, start, goal)) break;
-  }
-  V3 gc = sphere2cart(goal);
-  __syncwarp();
-  if (lane == 0) {
-    for (int i = 0; i < 3; ++i) { gs[DWBC_GS_DELTA_ORN + i] = d[i]; gs[DWBC_GS_GOAL_ORN + i] = o[i]; }
-    gs[DWBC_GS_START_SPH] = start.x; gs[DWBC_GS_START_SPH + 1] = start.y; gs[DWBC_GS_START_SPH + 2] = start.z;
-    gs[DWBC_GS_GOAL_SPH] = goal.x; gs[DWBC_GS_GOAL_SPH + 1] = goal.y; gs[DWBC_GS_GOAL_SPH + 2] = goal.z;
-    gs[DWBC_GS_GOAL_CART] = gc.x; gs[DWBC_GS_GOAL_CART + 1] = gc.y; gs[DWBC_GS_GOAL_CART + 2] = gc.z;
-    gs[DWBC_GS_GOAL_TIMER] = 0.0f;
-  }
-  __syncwarp();
-}
-
-// WG:831-843
-__device__ void resample_commands(const DwbcEnvCfg& cfg, const DwbcStepArgs& A, const Rng& rng, float* gs, int col, int lane) {
-  float cx = A.lin_vel_x[1] * rng(col) + A.lin_vel_x[0];
-  float cy = A.ang_vel_yaw[1] * rng(col + 1) + A.ang_vel_yaw[0];
-  float keep = (cx > cfg.lin_vel_x_clip || fabsf(cy) > cfg.ang_vel_yaw_clip) ? 1.0f : 0.0f;
-  __syncwarp();
-  if (lane == 0) { gs[0] = cx * keep; gs[1] = 0.0f * keep; gs[2] = cy * keep; }
-  __syncwarp();
-}
-
-struct TermCtx {
-  const DwbcEnvCfg& cfg;
-  float* sm;        // staging block
-  int lane, nd, na;
-  float root_z;
-  bool reset, time_out;
-  float mean_height_gap;  // mean(root_z - measured_heights) (LR:846) when heights are measured
-};
-
-// One reward term for the env of this warp (value identical on all lanes).  Side effects on
-// episode_metric_sums (WG:162-167) go to sm[S_SUM + n_sum_slots + metric].
-__device__ float eval_term(int term, const TermCtx& c) {
-  const DwbcEnvCfg& cfg = c.cfg;
-  float* sm = c.sm;
-  const int lane = c.lane, nd = c.nd, na = c.na;
-  const float tq = lane < nd ? sm[S_TQ + lane] : 0.0f;
-  const float dv = lane < nd ? sm[S_DOF + 2 * lane + 1] : 0.0f;
-  const float dp = lane < nd ? sm[S_DOF + 2 * lane] : 0.0f;
-  const float act = lane < na ? sm[S_ACT + lane] : 0.0f;
-  const float* gs = sm + S_GS;
-  const float* ds = sm + S_DS;
-  float* met = sm + S_SUM + cfg.n_sum_slots;
-  const bool l0 = lane == 0;
-  float r = 0.0f;
-  switch (term) {
-    case DWBC_TERM_energy_square: {  // WG:1466-1469
-      float e = lane < 12 ? tq * dv : 0.0f;
-      r = warp_sum(e * e);
-      if (l0) met[8] += r;
-    } break;
-    case DWBC_TERM_foot_contacts_z: {  // WG:1455-1458
-      float f = lane < 4 ? sm[S_FS + 6 * lane + 2] : 0.0f;
-      r = warp_sum(f * f);
-      if (l0) met[9] += r;
-    } break;
-    case DWBC_TERM_hip_action_l2: {  // WG:1379-1382
-      float a = (lane < 12 && lane % 3 == 0) ? act : 0.0f;
-      r = warp_sum(a * a);
-      if (l0) met[6] += r;
-    } break;
-    case DWBC_TERM_leg_action_l2: {  // WG:1405-1408
-      float a = lane < 12 ? act : 0.0f;
-      r = warp_sum(a * a);
-      if (l0) met[6] += r;
-    } break;
-    case DWBC_TERM_survive: r = 1.0f; break;  // WG:1452-1453
-    case DWBC_TERM_tracking_ang_vel_yaw_exp: {  // WG:1441-1444
-      float e = fabsf(gs[2] - ds[DWBC_DS_BASE_ANG_VEL + 2]);
-      if (l0) met[2] += e;
-      r = nexp(-e / cfg.tracking_sigma);
-    } break;
-    case DWBC_TERM_tracking_ang_vel_yaw_l1: {  // WG:1437-1439
-      float e = fabsf(gs[2] - ds[DWBC_DS_BASE_ANG_VEL + 2]);
-      r = -e + fabsf(gs[2]);
-    } break;
-    case DWBC_TERM_tracking_lin_vel_x_l1: {  // WG:1427-1430
-      float e = fabsf(gs[0] - ds[DWBC_DS_BASE_LIN_VEL]);
-      if (l0) met[1] += e;
-      r = -e + fabsf(gs[0]);
-    } break;
-    case DWBC_TERM_tracking_lin_vel_x_exp: {  // WG:1432-1435
-      float e = fabsf(gs[0] - ds[DWBC_DS_BASE_LIN_VEL]);
-      if (l0) met[1] += e;
-      r = nexp(-e / cfg.tracking_sigma);
-    } break;
-    case DWBC_TERM_tracking_lin_vel_y_l2: { float e = gs[1] - ds[DWBC_DS_BASE_LIN_VEL + 1]; r = e * e; } break;  // WG:1446
-    case DWBC_TERM_tracking_lin_vel_z_l2: { float e = gs[2] - ds[DWBC_DS_BASE_LIN_VEL + 2]; r = e * e; } break;  // WG:1449
-    case DWBC_TERM_tracking_lin_vel: {  // WG:1422-1425
-      float ex = gs[0] - ds[DWBC_DS_BASE_LIN_VEL], ey = gs[1] - ds[DWBC_DS_BASE_LIN_VEL + 1];
-      r = nexp(-(ex * ex + ey * ey) / cfg.tracking_sigma);
-    } break;
-    case DWBC_TERM_tracking_ang_vel: {  // LR:886-889
-      float e = gs[2] - ds[DWBC_DS_BASE_ANG_VEL + 2];
-      r = nexp(-(e * e) / cfg.tracking_sigma);
-    } break;
-    case DWBC_TERM_torques: {  // WG:1460-1464
-      r = warp_sum(tq * tq);
-      if (l0) met[7] += r;
-    } break;
-    case DWBC_TERM_leg_energy_abs_sum: {  // WG:1396-1399
-      r = warp_sum(lane < 12 ? fabsf(tq * dv) : 0.0f);
-      if (l0) met[0] += r;
-    } break;
-    case DWBC_TERM_leg_energy_sum_abs: r = fabsf(warp_sum(lane < 12 ? tq * dv : 0.0f)); break;  // WG:1401-1403
-    case DWBC_TERM_leg_energy: r = warp_sum(lane < 12 ? tq * dv : 0.0f); break;                 // WG:1410-1412
-    case DWBC_TERM_arm_energy_abs_sum: r = warp_sum((lane >= 12 && lane < nd - 2) ? fabsf(tq * dv) : 0.0f); break;  // WG:1414
-    case DWBC_TERM_tracking_ee_sphere: {  // WG:1352-1358
-      V3 d = mk(sm[S_EE] - sm[S_ROOT], sm[S_EE + 1] - sm[S_ROOT + 1], sm[S_EE + 2] - cfg.z_invariant_offset);
-      V3 s = cart2sphere(quat_rotate_inverse(ds + DWBC_DS_YAW_QUAT, d));
-      float e = (fabsf(s.x - gs[DWBC_GS_CURR_SPH]) * cfg.sphere_error_scale[0] +
-                 fabsf(s.y - gs[DWBC_GS_CURR_SPH + 1]) * cfg.sphere_error_scale[1]) +
-                fabsf(s.z - gs[DWBC_GS_CURR_SPH + 2]) * cfg.sphere_error_scale[2];
-      if (l0) met[4] += e;
-      r = nexp(-e / cfg.tracking_ee_sigma);
-    } break;
-    case DWBC_TERM_tracking_ee_cart: {  // WG:1360-1366
-      V3 t = quat_apply(ds + DWBC_DS_YAW_QUAT, mk(gs[DWBC_GS_CURR_CART], gs[DWBC_GS_CURR_CART + 1], gs[DWBC_GS_CURR_CART + 2]));
-      float e = (fabsf(sm[S_EE] - (sm[S_ROOT] + t.x)) + fabsf(sm[S_EE + 1] - (sm[S_ROOT + 1] + t.y))) +
-                fabsf(sm[S_EE + 2] - (cfg.z_invariant_offset + t.z));
-      if (l0) met[3] += e;
-      r = nexp(-e / cfg.tracking_ee_sigma);
-    } break;
-    case DWBC_TERM_tracking_ee_orn:
-    case DWBC_TERM_tracking_ee_orn_ry: {  // WG:1368-1394
-      float eu[3];
-      euler_from_quat(sm + S_EE + 3, eu[0], eu[1], eu[2]);
-      float d0 = wrap_pi(gs[DWBC_GS_GOAL_ORN] - eu[0]), d1 = wrap_pi(gs[DWBC_GS_GOAL_ORN + 1] - eu[1]),
-            d2 = wrap_pi(gs[DWBC_GS_GOAL_ORN + 2] - eu[2]);
-      float e;
-      if (term == DWBC_TERM_tracking_ee_orn) {
-        e = (fabsf(d0) * cfg.orn_error_scale[0] + fabsf(d1) * cfg.orn_error_scale[1]) + fabsf(d2) * cfg.orn_error_scale[2];
-      } else {
-        e = fabsf(d0 * cfg.orn_error_scale[0]) + fabsf(d2 * cfg.orn_error_scale[2]);
-        if (l0) met[5] += e;
-      }
-      r = nexp(-e / cfg.tracking_ee_sigma);
-    } break;
-    case DWBC_TERM_lin_vel_z: r = ds[DWBC_DS_BASE_LIN_VEL + 2] * ds[DWBC_DS_BASE_LIN_VEL + 2]; break;  // LR:832
-    case DWBC_TERM_ang_vel_xy:  // LR:836
-      r = ds[DWBC_DS_BASE_ANG_VEL] * ds[DWBC_DS_BASE_ANG_VEL] + ds[DWBC_DS_BASE_ANG_VEL + 1] * ds[DWBC_DS_BASE_ANG_VEL + 1];
-      break;
-    case DWBC_TERM_base_height: { float g = c.mean_height_gap - cfg.base_height_target; r = g * g; } break;  // LR:844-847
-    case DWBC_TERM_dof_vel: r = warp_sum(dv * dv); break;                                                  // LR:853
-    case DWBC_TERM_dof_acc: {  // LR:857-859
-      float a = lane < nd ? (ds[DWBC_DS_LAST_DOF_VEL + lane] - dv) / cfg.dt : 0.0f;
-      r = warp_sum(a * a);
-    } break;
-    case DWBC_TERM_action_rate: {  // LR:861-863
-      float a = lane < na ? ds[DWBC_DS_LAST_ACTIONS + lane] - act : 0.0f;
-      r = warp_sum(a * a);
-    } break;
-    case DWBC_TERM_collision: {  // LR:865-867
-      float v = 0.0f;
-      if (lane < cfg.n_penalized) {
-        const float* f = sm + S_CF + 3 * (4 + lane);
-        v = sqrtf((f[0] * f[0] + f[1] * f[1]) + f[2] * f[2]) > 0.1f ? 1.0f : 0.0f;
-      }
-      r = warp_sum(v);
-    } break;
-    case DWBC_TERM_termination: r = (c.reset && !c.time_out) ? 1.0f : 0.0f; break;  // LR:869-871
-    case DWBC_TERM_dof_pos_limits: {  // LR:873-877
-      float o = 0.0f;
-      if (lane < nd) o = -fminf(dp - cfg.dof_pos_lower[lane], 0.0f) + fmaxf(dp - cfg.dof_pos_upper[lane], 0.0f);
-      r = warp_sum(o);
-    } break;
-    case DWBC_TERM_dof_vel_limits:  // LR:879-882
-      r = warp_sum(lane < nd ? clipf(fabsf(dv) - cfg.dof_vel_limits[lane] * cfg.soft_dof_vel_limit, 0.0f, 1.0f) : 0.0f);
-      break;
-    case DWBC_TERM_torque_limits:  // LR:884-886
-      r = warp_sum(lane < nd ? fmaxf(fabsf(tq) - cfg.torque_limits[lane] * cfg.soft_torque_limit, 0.0f) : 0.0f);
-      break;
-    case DWBC_TERM_feet_air_time: {  // LR:896-908 (stateful: feet_air_time, last_contacts)
-      float v = 0.0f;
-      if (lane < 4) {
-        bool contact = sm[S_CF + 3 * lane + 2] > 1.0f;
-        bool filt = contact || (sm[S_DS + DWBC_DS_LAST_CONTACTS + lane] != 0.0f);
-        float fat = sm[S_DS + DWBC_DS_FEET_AIR_TIME + lane];
-        bool first = (fat > 0.0f) && filt;
-        fat += cfg.dt;
-        v = (fat - 0.5f) * (first ? 1.0f : 0.0f);
-        sm[S_DS + DWBC_DS_LAST_CONTACTS + lane] = contact ? 1.0f : 0.0f;
-        sm[S_DS + DWBC_DS_FEET_AIR_TIME + lane] = fat * (filt ? 0.0f : 1.0f);
-      }
-      r = warp_sum(v) * ((sqrtf(gs[0] * gs[0] + gs[1] * gs[1]) > 0.1f) ? 1.0f : 0.0f);
-      __syncwarp();
-    } break;
-    case DWBC_TERM_stumble: {  // LR:910-913
-      bool s = false;
-      if (lane < 4) {
-        const float* f = sm + S_CF + 3 * lane;
-        s = sqrtf(f[0] * f[0] + f[1] * f[1]) > 5.0f * fabsf(f[2]);
-      }
-      r = __any_sync(FULL, s) ? 1.0f : 0.0f;
-    } break;
-    case DWBC_TERM_stand_still: {  // LR:915-917
-      float s = warp_sum(lane < nd ? fabsf(dp - cfg.default_dof_pos[lane]) : 0.0f);
-      r = s * ((sqrtf(gs[0] * gs[0] + gs[1] * gs[1]) < 0.1f) ? 1.0f : 0.0f);
-    } break;
-    case DWBC_TERM_feet_contact_forces: {  // LR:919-921
-      float v = 0.0f;
-      if (lane < 4) {
-        const float* f = sm + S_CF + 3 * lane;
-        v = fmaxf(sqrtf((f[0] * f[0] + f[1] * f[1]) + f[2] * f[2]) - cfg.max_contact_force, 0.0f);
-      }
-      r = warp_sum(v);
-    } break;
-    default: break;
-  }
-  return r;
-}
+static_assert(S_DOF - S_ROOT >= 26 && S_EE - S_DOF >= 2 * DWBC_MAX_DOF && S_GS - S_AH >= 8 * DWBC_MAX_DOF && S_SUM - S_DS >= DWBC_DS &&
+                  S_PRIV - S_SUM >= DWBC_MAX_SLOTS && S_MASS - S_CF >= 3 * (4 + 2 * DWBC_MAX_IDX) && S_RP - S_FEAT >= FE_COUNT,
+              "staging rows overlap");
 
 // kLong = false: the history row (<= 1024 floats) is loaded into registers before anything else and re-emitted from there.
 // kLong = true (history_len * num_prop > 1024, e.g. 20 or 50 steps of 76): the row is streamed at the end instead, in ascending
 // 32-float4 chunks: each chunk is loaded, written to obs clipped (WG:992, 1195-1196), and after a __syncwarp written back one num_prop
 // row lower (WG:997-999).  In place is safe: the targets of chunk i lie below its end, so chunks <= i have read them already.
+// The minimum of 1 CTA per SM keeps ptxas from capping the streaming form at 64 registers, where it spills.
 template <bool kLong>
-__global__ void __launch_bounds__(ENV_WARPS * 32)
+__global__ void __launch_bounds__(ENV_WARPS * 32, 1)
 env_step_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant__ DwbcEnvBuffers B,
                 const __grid_constant__ DwbcStepArgs A) {
   __shared__ __align__(16) float smem[ENV_WARPS * S_TOTAL];
@@ -273,7 +45,7 @@ env_step_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant__ 
   const int e = blockIdx.x * ENV_WARPS + wid;
   if (e >= cfg.num_envs) return;
   float* sm = smem + wid * S_TOTAL;
-  const int nd = cfg.num_dofs, na = cfg.num_actions, P = cfg.num_prop, H = cfg.history_len;
+  const int nd = cfg.num_dofs, na = cfg.num_actions, ahl = cfg.action_hist_len, P = cfg.num_prop, H = cfg.history_len;
   const int nbp1 = cfg.num_bodies_p1;
   const int nh4 = (H * P) >> 2, p4 = P >> 2, pp4 = (P + cfg.num_priv) >> 2;
   const int nslots = cfg.n_sum_slots + DWBC_NUM_METRICS;
@@ -281,7 +53,6 @@ env_step_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant__ 
   // ---- 1. history row: all 128-bit loads in flight first --------------------------------------
   float4* hist4 = reinterpret_cast<float4*>(B.obs_history + (size_t)e * H * P);
   float4 h[kLong ? 1 : MAX_H4];
-  bool hist_zeroed = false;                  // (kLong) reset this step: the old history reads as zeros (WG:735)
   if constexpr (!kLong) {
 #pragma unroll
     for (int i = 0; i < MAX_H4; ++i) {
@@ -289,26 +60,26 @@ env_step_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant__ 
       h[i] = idx < nh4 ? ldg_stream(hist4 + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
   }
-  // ---- 2. coalesced staging of the env's small inputs ------------------------------------------
+  // ---- 2. coalesced staging of the env's rows ----------------------------------------------------
   float* root_g = B.root_states + (size_t)e * 26;
-  if (lane < 13) sm[S_ROOT + lane] = root_g[lane];
+  if (lane < 26) sm[S_ROOT + lane] = root_g[lane];
   float* dof_g = B.dof_state + (size_t)e * 2 * nd;
   for (int i = lane; i < 2 * nd; i += 32) sm[S_DOF + i] = dof_g[i];
-  if (lane < 13) sm[S_EE + lane] = __ldg(B.rigid_body_state + ((size_t)e * nbp1 + cfg.gripper_idx) * 13 + lane);
+  if (lane < 7) sm[S_EE + lane] = __ldg(B.rigid_body_state + ((size_t)e * nbp1 + cfg.gripper_idx) * 13 + lane);
   if (lane < 24) sm[S_FS + lane] = __ldg(B.force_sensor + (size_t)e * 24 + lane);
   if (lane < nd) sm[S_TQ + lane] = __ldg(B.torques + (size_t)e * nd + lane);
   if (lane < na) sm[S_ACT + lane] = __ldg(B.actions + (size_t)e * na + lane);
-  float* ah_g = B.action_history + (size_t)e * cfg.action_hist_len * na;
-  if (lane < na) sm[S_AH + lane] = ah_g[(cfg.action_hist_len - 1) * na + lane];
+  float* ah_g = B.action_history + (size_t)e * ahl * na;
+  for (int i = lane; i < ahl * na; i += 32) sm[S_AH + i] = ah_g[i];
   float* gs_g = B.goal_state + (size_t)e * DWBC_GS;
   if (lane < DWBC_GS) sm[S_GS + lane] = gs_g[lane];
   float* ds_g = B.derived_state + (size_t)e * DWBC_DS;
-  for (int i = DWBC_DS_FEET_AIR_TIME + lane; i < DWBC_DS; i += 32) sm[S_DS + i] = ds_g[i];
+  for (int i = DWBC_DS_FEET_AIR_TIME + lane; i < DWBC_DS; i += 32) sm[S_DS + i] = ds_g[i];   // columns below are rewritten every step
   float* sum_g = B.episode_sums + (size_t)e * cfg.sums_stride;
   for (int i = lane; i < nslots; i += 32) sm[S_SUM + i] = sum_g[i];
-  if (lane < 5) sm[S_PRIV + lane] = __ldg(B.mass_params + (size_t)e * 5 + lane);
-  else if (lane == 5) sm[S_PRIV + 5] = __ldg(B.friction + e);
-  if (lane < na) sm[S_PRIV + 6 + lane] = __ldg(B.motor_strength + (size_t)e * na + lane) - 1.0f;
+  if (lane < 5) sm[S_MASS + lane] = __ldg(B.mass_params + (size_t)e * 5 + lane);
+  else if (lane == 5) sm[S_FRIC] = __ldg(B.friction + e);
+  if (lane < na) sm[S_MOTOR + lane] = __ldg(B.motor_strength + (size_t)e * na + lane);
   {
     const int ncf = 4 + cfg.n_penalized + cfg.n_term_contact;
     for (int i = lane; i < 3 * ncf; i += 32) {
@@ -319,233 +90,42 @@ env_step_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant__ 
   }
   long long ep = B.episode_length[e] + 1;  // WG:875
   __syncwarp();
+  const EnvView v{sm + S_ROOT, sm + S_DOF, sm + S_FS, sm + S_TQ, sm + S_ACT, sm + S_AH, sm + S_GS, sm + S_DS, sm + S_SUM, sm + S_EE,
+                  sm + S_CF, sm + S_MASS, sm + S_FRIC, sm + S_MOTOR, sm + S_PROP, sm + S_PRIV, sm + S_FEAT, sm + S_RP, sm + S_REW};
 
-  Rng rng{A.rand_uniform, A.seed, A.step, e};
-  float* gs = sm + S_GS;
-  float* ds = sm + S_DS;
-
-  // ---- 3. derived base state (WG:879-884) -------------------------------------------------------
-  float yaw;
-  {
-    const float* q = sm + S_ROOT + 3;
-    V3 blv = quat_rotate_inverse(q, mk(sm[S_ROOT + 7], sm[S_ROOT + 8], sm[S_ROOT + 9]));
-    V3 bav = quat_rotate_inverse(q, mk(sm[S_ROOT + 10], sm[S_ROOT + 11], sm[S_ROOT + 12]));
-    float r0, p0;
-    euler_from_quat(q, r0, p0, yaw);
-    float cy = ncos(yaw * 0.5f), sy = nsin(yaw * 0.5f);
-    __syncwarp();
-    if (lane == 0) {
-      ds[DWBC_DS_BASE_LIN_VEL] = blv.x; ds[DWBC_DS_BASE_LIN_VEL + 1] = blv.y; ds[DWBC_DS_BASE_LIN_VEL + 2] = blv.z;
-      ds[DWBC_DS_BASE_ANG_VEL] = bav.x; ds[DWBC_DS_BASE_ANG_VEL + 1] = bav.y; ds[DWBC_DS_BASE_ANG_VEL + 2] = bav.z;
-      ds[DWBC_DS_YAW_EULER] = 0.0f; ds[DWBC_DS_YAW_EULER + 1] = 0.0f; ds[DWBC_DS_YAW_EULER + 2] = yaw;
-      ds[DWBC_DS_YAW_QUAT] = 0.0f; ds[DWBC_DS_YAW_QUAT + 1] = 0.0f; ds[DWBC_DS_YAW_QUAT + 2] = sy; ds[DWBC_DS_YAW_QUAT + 3] = cy;
-    }
-    __syncwarp();
-  }
-  // ---- 4. EE goal interpolation + timer (WG:1344-1350) ------------------------------------------
-  {
-    float t = clipf(gs[DWBC_GS_GOAL_TIMER] / gs[DWBC_GS_TRAJ_T], 0.0f, 1.0f);
-    V3 cs = lerp3(mk(gs[DWBC_GS_START_SPH], gs[DWBC_GS_START_SPH + 1], gs[DWBC_GS_START_SPH + 2]),
-                  mk(gs[DWBC_GS_GOAL_SPH], gs[DWBC_GS_GOAL_SPH + 1], gs[DWBC_GS_GOAL_SPH + 2]), t);
-    V3 cc = sphere2cart(cs);
-    float timer = gs[DWBC_GS_GOAL_TIMER] + 1.0f;
-    bool expired = timer > gs[DWBC_GS_TRAJ_TOTAL];
-    __syncwarp();
-    if (lane == 0) {
-      gs[DWBC_GS_CURR_SPH] = cs.x; gs[DWBC_GS_CURR_SPH + 1] = cs.y; gs[DWBC_GS_CURR_SPH + 2] = cs.z;
-      gs[DWBC_GS_CURR_CART] = cc.x; gs[DWBC_GS_CURR_CART + 1] = cc.y; gs[DWBC_GS_CURR_CART + 2] = cc.z;
-      gs[DWBC_GS_GOAL_TIMER] = timer;
-    }
-    __syncwarp();
-    if (expired) resample_goal(cfg, A, rng, gs, yaw, DWBC_RAND_GOAL_ORN, DWBC_RAND_GOAL_SPH, lane);
-  }
-  // ---- 5. callback: command resampling, height scan, push (WG:917-935) --------------------------
-  if (ep % cfg.resample_interval == 0) resample_commands(cfg, A, rng, gs, DWBC_RAND_CMD, lane);
-  float mean_gap = 0.0f;
-  if (cfg.measure_heights) {  // LR:793-829
-    const int npts = cfg.n_height_x * cfg.n_height_y;
-    float qy[4] = {0.0f, 0.0f, sm[S_ROOT + 5], sm[S_ROOT + 6]};
-    float n = fmaxf(sqrtf(qy[2] * qy[2] + qy[3] * qy[3]), 1e-9f);  // utils/math.py:38-42 + normalize()
-    qy[2] = qy[2] / n; qy[3] = qy[3] / n;
-    float gap = 0.0f;
-    for (int i = lane; i < npts; i += 32) {
-      int ix = i / cfg.n_height_y, iy = i - ix * cfg.n_height_y;
-      V3 pt = quat_apply(qy, mk(cfg.height_x[ix], cfg.height_y[iy], 0.0f));
-      float fx = ((pt.x + sm[S_ROOT]) + cfg.border_size) / cfg.horizontal_scale;
-      float fy = ((pt.y + sm[S_ROOT + 1]) + cfg.border_size) / cfg.horizontal_scale;
-      long long px = (long long)fx, py = (long long)fy;  // .long(): truncation toward zero
-      px = px < 0 ? 0 : (px > cfg.terrain_rows - 2 ? cfg.terrain_rows - 2 : px);
-      py = py < 0 ? 0 : (py > cfg.terrain_cols - 2 ? cfg.terrain_cols - 2 : py);
-      const int16_t* hs = B.height_samples + px * cfg.terrain_cols + py;
-      int16_t m = min(min(__ldg(hs), __ldg(hs + cfg.terrain_cols)), __ldg(hs + 1));
-      float hgt = (float)m * cfg.vertical_scale;
-      B.measured_heights[(size_t)e * npts + i] = hgt;
-      gap += sm[S_ROOT + 2] - hgt;
-    }
-    mean_gap = warp_sum(gap) / (float)npts;
-  }
-  bool root_dirty = false;
-  if (A.do_push) {  // WG:804-814
-    float vx = cfg.push_vel[1] * rng(DWBC_RAND_PUSH) + cfg.push_vel[0];
-    float vy = cfg.push_vel[1] * rng(DWBC_RAND_PUSH + 1) + cfg.push_vel[0];
-    if (((gs[0] + gs[1]) + gs[2]) == 0.0f) { vx *= 2.5f; vy *= 2.5f; }
-    __syncwarp();
-    if (lane == 0) { sm[S_ROOT + 7] = vx; sm[S_ROOT + 8] = vy; }
-    __syncwarp();
-    root_dirty = true;
-  }
-  // ---- 6. termination (WG:937-963) ---------------------------------------------------------------
-  bool time_out, reset;
-  {
-    bool contact = false;
-    for (int i = 0; i < cfg.n_term_contact; ++i) {
-      const float* f = sm + S_CF + 3 * (4 + cfg.n_penalized + i);
-      contact = contact || (sqrtf((f[0] * f[0] + f[1] * f[1]) + f[2] * f[2]) > 1.0f);
-    }
-    float r0, p0, y0;
-    euler_from_quat(sm + S_ROOT + 3, r0, p0, y0);
-    const float* g = gs + (cfg.goal_is_cart ? DWBC_GS_CURR_CART : DWBC_GS_CURR_SPH);
-    bool r_bad = ((r0 > cfg.term_roll) && (g[2] >= 0.0f)) || ((r0 < -cfg.term_roll) && (g[2] <= 0.0f));
-    bool p_bad = ((p0 > cfg.term_pitch) && (g[1] >= 0.0f)) || ((p0 < -cfg.term_pitch) && (g[1] <= 0.0f));
-    bool z_bad = sm[S_ROOT + 2] < cfg.term_z;
-    time_out = ep > cfg.max_episode_length;
-    reset = contact || r_bad || p_bad || z_bad || time_out;
-  }
-  // ---- 7. rewards (WG:170-205) -------------------------------------------------------------------
-  float rew[2];
-  {
-    TermCtx ctx{cfg, sm, lane, nd, na, sm[S_ROOT + 2], reset, time_out, mean_gap};
-#pragma unroll
-    for (int ch = 0; ch < 2; ++ch) {
-      const int n = ch == 0 ? cfg.n_leg_terms : cfg.n_arm_terms;
-      const int32_t* terms = ch == 0 ? cfg.leg_term : cfg.arm_term;
-      const int32_t* slots = ch == 0 ? cfg.leg_slot : cfg.arm_slot;
-      const float* scales = ch == 0 ? A.leg_scale : A.arm_scale;
-      float buf = 0.0f;
-      for (int i = 0; i < n; ++i) {
-        float r = eval_term(terms[i], ctx) * scales[i];
-        buf += r;
-        if (lane == 0) sm[S_SUM + slots[i]] += r;
-      }
-      if (cfg.only_positive_rewards) buf = fmaxf(buf, 0.0f);
-      float ts = ch == 0 ? A.leg_termination_scale : A.arm_termination_scale;
-      if (ts != 0.0f && cfg.termination_slot >= 0) {
-        float r = ((reset && !time_out) ? 1.0f : 0.0f) * ts;
-        buf += r;
-        if (lane == 0) sm[S_SUM + cfg.termination_slot] += r;
-      }
-      rew[ch] = buf / 100.0f;
-    }
-    __syncwarp();
-  }
-  // ---- 8. reset (WG:695-754) ---------------------------------------------------------------------
-  if (reset) {
-    if (cfg.terrain_curriculum) {  // LR:421-441 (base-class semantics, SURVEY a21)
-      float* org = B.env_origins + (size_t)e * 3;
-      float dx = sm[S_ROOT] - org[0], dy = sm[S_ROOT + 1] - org[1];
-      float dist = sqrtf(dx * dx + dy * dy);
-      bool up = dist > cfg.terrain_env_length / 2.0f;
-      bool down = (dist < sqrtf(gs[0] * gs[0] + gs[1] * gs[1]) * cfg.max_episode_length_s * 0.5f) && !up;
-      long long lvl = B.terrain_levels[e] + (up ? 1 : 0) - (down ? 1 : 0);
-      if (lvl >= cfg.max_terrain_level) {
-        long long rl = (long long)(rng(DWBC_RAND_TERRAIN) * (float)cfg.max_terrain_level);
-        lvl = rl > cfg.max_terrain_level - 1 ? cfg.max_terrain_level - 1 : rl;
-      } else if (lvl < 0) {
-        lvl = 0;
-      }
-      const float* to = B.terrain_origins + ((size_t)lvl * cfg.terrain_n_types + B.terrain_types[e]) * 3;
-      float o0 = to[0], o1 = to[1], o2 = to[2];
-      __syncwarp();
-      if (lane == 0) { B.terrain_levels[e] = lvl; org[0] = o0; org[1] = o1; org[2] = o2; }
-      __syncwarp();
-    }
-    // _reset_dofs WG:816-828
-    if (lane < nd) {
-      float pos = cfg.default_dof_pos[lane] * (cfg.dof_reset[1] * rng(DWBC_RAND_RST_DOF + lane) + cfg.dof_reset[0]);
-      sm[S_DOF + 2 * lane] = pos;
-      sm[S_DOF + 2 * lane + 1] = 0.0f;
-    }
-    // _reset_root_states WG:757-788
-    if (lane < 13) {
-      float v = cfg.base_init_state[lane];
-      if (lane < 3) v += B.env_origins[(size_t)e * 3 + lane];
-      if (lane < 2) v += cfg.origin_perturb[1] * rng(DWBC_RAND_RST_XY + lane) + cfg.origin_perturb[0];
-      if (lane >= 7) v = cfg.init_vel_perturb[1] * rng(DWBC_RAND_RST_VEL + lane - 7) + cfg.init_vel_perturb[0];
-      sm[S_ROOT + lane] = v;
-    }
-    __syncwarp();
-    for (int i = lane; i < 2 * nd; i += 32) dof_g[i] = sm[S_DOF + i];
-    if (lane == 0) {
-      root_g[13] = cfg.box_x;
-      root_g[14] = sm[S_ROOT + 1] + B.box_env_origins_delta_y[e];
-      root_g[15] = cfg.box_z;
-    }
-    root_dirty = true;
-    if (time_out) resample_commands(cfg, A, rng, gs, DWBC_RAND_RST_CMD, lane);  // WG:723-727
-    resample_goal(cfg, A, rng, gs, yaw, DWBC_RAND_RST_GOAL_ORN, DWBC_RAND_RST_GOAL_SPH, lane);
-    // buffers WG:732-740
-    if (lane < 4) sm[S_DS + DWBC_DS_FEET_AIR_TIME + lane] = 0.0f;
-    if (lane < na) sm[S_AH + lane] = 0.0f;
-    for (int i = lane; i < cfg.action_hist_len * na; i += 32) ah_g[i] = 0.0f;
+  // ---- 3. DOF reductions, height scan, then the scalar step on lane 0 -----------------------------
+  dof_features(cfg, v, feature_mask(cfg), cfg.default_dof_pos, nd, na, lane);
+  const float gap = cfg.measure_heights ? height_scan(cfg, B, v.root, e, lane) : 0.0f;
+  if (lane == 0) v.rp[3] = gap;
+  __syncwarp();
+  int flags = 0;
+  if (lane == 0) flags = scalar_step(cfg, A, v, e, ep);
+  __syncwarp();   // orders lane 0's writes to the staged rows before the warp's reads and writes in fix_up() (a shuffle does not)
+  flags = __shfl_sync(FULL, flags, 0);
+  // ---- 4. goal resample and reset -----------------------------------------------------------------
+  if (flags & (F_GOAL_RS | F_RESET)) flags = fix_up(cfg, A, B, v, flags, e, nd, na, ahl, nslots, lane);
+  if (flags & F_RESET) {
+    ep = 0;
     if constexpr (!kLong) {
 #pragma unroll
-      for (int i = 0; i < MAX_H4; ++i) h[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    } else {
-      hist_zeroed = true;
+      for (int i = 0; i < MAX_H4; ++i) h[i] = make_float4(0.f, 0.f, 0.f, 0.f);   // the old history reads as zeros (WG:735)
     }
-    ep = 0;
-    // extras['episode'] means (WG:743-750): the ended episode's sums go to this env's slot; episode_stats_kernel adds them up
-    for (int i = lane; i < nslots; i += 32) {
-      B.episode_scratch[(size_t)e * cfg.sums_stride + i] = sm[S_SUM + i];
-      sm[S_SUM + i] = 0.0f;
-    }
-    __syncwarp();
   }
-  if (root_dirty && lane < 13) root_g[lane] = sm[S_ROOT + lane];
+  __syncwarp();
 
-  // ---- 9. observations (WG:966-1001, column map SURVEY Appendix B) ------------------------------
-  {
-    float r0, p0, y0;
-    euler_from_quat(sm + S_ROOT + 3, r0, p0, y0);  // post-reset quaternion (base_quat is a view, WG:535)
-    float* prop = sm + S_PROP;
-    if (lane == 0) {
-      prop[0] = r0; prop[1] = p0;
-      for (int i = 0; i < 3; ++i) prop[2 + i] = ds[DWBC_DS_BASE_ANG_VEL + i] * cfg.obs_scale_ang_vel;
-    }
-    if (lane < nd) {
-      int d = cfg.ig2raisim[lane];
-      float pos = sm[S_DOF + 2 * d];
-      if (d == cfg.waist_dof) pos = wrap_pi(pos);
-      prop[5 + lane] = (pos - cfg.default_dof_pos[d]) * cfg.obs_scale_dof_pos;
-      prop[5 + nd + lane] = sm[S_DOF + 2 * d + 1] * cfg.obs_scale_dof_vel;
-    }
-    if (lane < na) prop[5 + 2 * nd + lane] = sm[S_AH + cfg.ig2raisim[lane]];
-    const int o = 5 + 2 * nd + na;
-    if (lane < 4) {
-      const float* f = sm + S_FS + 6 * cfg.feet_perm[lane];
-      float nrm = sqrtf(((((f[0] * f[0] + f[1] * f[1]) + f[2] * f[2]) + f[3] * f[3]) + f[4] * f[4]) + f[5] * f[5]);
-      prop[o + lane] = nrm > 1.5f ? 1.0f : 0.0f;
-    }
-    if (lane == 31) {
-      prop[o + 4] = gs[0] * cfg.obs_scale_lin_vel;
-      prop[o + 5] = gs[1] * cfg.obs_scale_lin_vel;
-      prop[o + 6] = gs[2] * cfg.obs_scale_ang_vel;
-      const float* g = gs + (cfg.goal_is_cart ? DWBC_GS_CURR_CART : DWBC_GS_CURR_SPH);
-      for (int i = 0; i < 3; ++i) { prop[o + 7 + i] = g[i]; prop[o + 10 + i] = gs[DWBC_GS_DELTA_ORN + i]; }
-    }
-    // tail copies WG:908-910
-    if (lane < na) ds[DWBC_DS_LAST_ACTIONS + lane] = sm[S_ACT + lane];
-    if (lane < nd) ds[DWBC_DS_LAST_DOF_VEL + lane] = sm[S_DOF + 2 * lane + 1];
-    if (lane < 6) ds[DWBC_DS_LAST_ROOT_VEL + lane] = sm[S_ROOT + 7 + lane];
-    if (lane == 7) ds[27] = 0.0f;  // DWBC_DS_OOB_AGE (v2 fast-path bookkeeping): v1 always clips, stay conservative
-    __syncwarp();
-  }
-  // ---- 10. outputs -------------------------------------------------------------------------------
+  // ---- 5. observations (WG:966-1001); this kernel always writes them clipped ----------------------
+  assemble_obs(cfg, v, 0, cfg.ig2raisim, cfg.default_dof_pos, INFINITY, nd, na, ahl, lane);
+  assemble_obs(cfg, v, 1, cfg.ig2raisim, cfg.default_dof_pos, INFINITY, nd, na, ahl, lane);
+  if (lane == 0) v.ds[DWBC_DS_OOB_AGE] = 0.0f;   // no stored history row is known to lie within the clip
+  __syncwarp();
+
+  // ---- 6. outputs -------------------------------------------------------------------------------
   const float c = cfg.clip_obs > 0.0f ? cfg.clip_obs : INFINITY;
   float4* obs4 = reinterpret_cast<float4*>(B.obs_buf + (size_t)e * B.obs_stride);
   const float4* prop4 = reinterpret_cast<const float4*>(sm + S_PROP);
   const float4* priv4 = reinterpret_cast<const float4*>(sm + S_PRIV);
   if (lane < pp4) stg_stream(obs4 + lane, clip4(lane < p4 ? prop4[lane] : priv4[lane - p4], c));
+  const bool fill = (flags & F_FILL) != 0;
   if constexpr (!kLong) {
 #pragma unroll
     for (int i = 0; i < MAX_H4; ++i) {
@@ -553,7 +133,7 @@ env_step_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant__ 
       if (idx < nh4) stg_stream(obs4 + pp4 + idx, clip4(h[i], c));  // OLD history (WG:992)
     }
     __syncwarp();  // every lane's history loads have been consumed: the in-place shift below is safe
-    if (ep <= 1) {  // WG:994-996: fill all H rows with the new proprioception
+    if (fill) {     // WG:994-996: fill all H rows with the new proprioception
 #pragma unroll
       for (int i = 0; i < MAX_H4; ++i) {
         int idx = lane + 32 * i;
@@ -571,39 +151,30 @@ env_step_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant__ 
     const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int i0 = 0; i0 < nh4; i0 += 32) {
       const int idx = i0 + lane;
-      h[0] = idx < nh4 && !hist_zeroed ? __ldcs(hist4 + idx) : zero4;
+      h[0] = idx < nh4 && !(flags & F_RESET) ? __ldcs(hist4 + idx) : zero4;   // reset: the old history reads as zeros (WG:735)
       if (idx < nh4) stg_stream(obs4 + pp4 + idx, clip4(h[0], c));    // OLD history (WG:992)
       __syncwarp();  // the whole chunk has been read: its targets (and everything below them) may be overwritten
-      if (ep <= 1) {          // WG:994-996
+      if (fill) {             // WG:994-996
         if (idx < nh4) hist4[idx] = prop4[idx % p4];
       } else if (idx >= p4 && idx < nh4) {
         hist4[idx - p4] = h[0];                                            // WG:997-999
       }
     }
-    if (ep > 1 && lane < p4) hist4[nh4 - p4 + lane] = prop4[lane];          // WG:1000
+    if (!fill && lane < p4) hist4[nh4 - p4 + lane] = prop4[lane];          // WG:1000
+  }
+  if (flags & F_ROOT_DIRTY) { if (lane < 26) root_g[lane] = sm[S_ROOT + lane]; }
+  if (flags & F_DOF_DIRTY) {
+    for (int i = lane; i < 2 * nd; i += 32) dof_g[i] = sm[S_DOF + i];
+    for (int i = lane; i < ahl * na; i += 32) ah_g[i] = sm[S_AH + i];
   }
   if (lane < DWBC_GS) gs_g[lane] = sm[S_GS + lane];
   for (int i = lane; i < DWBC_DS; i += 32) ds_g[i] = sm[S_DS + i];
   for (int i = lane; i < nslots; i += 32) sum_g[i] = sm[S_SUM + i];
   if (lane == 0) {
     B.episode_length[e] = ep;
-    B.rew_buf[e] = rew[0];
-    B.arm_rew_buf[e] = rew[1];
-    B.reset_buf[e] = reset ? 1 : 0;
-    B.time_out_buf[e] = time_out ? 1 : 0;
-    if (B.store_rewards) {          // PPO.process_env_step's reward path (PPO:130-134) + dones (RS:102), straight into the storage rows
-      const float to = time_out ? 1.0f : 0.0f;
-      B.store_rewards[2 * (size_t)e] = rew[0] + B.store_gamma * (B.store_values[2 * (size_t)e] * to);
-      B.store_rewards[2 * (size_t)e + 1] = rew[1] + B.store_gamma * (B.store_values[2 * (size_t)e + 1] * to);
-      if (B.store_dones) B.store_dones[e] = reset ? 1 : 0;
-    }
+    store_step(B, e, flags, v.rew[0], v.rew[1]);
   }
-  if (cfg.measure_heights && B.heights_obs) {  // LR:221-223
-    const int npts = cfg.n_height_x * cfg.n_height_y;
-    for (int i = lane; i < npts; i += 32)
-      B.heights_obs[(size_t)e * npts + i] =
-          clipf((sm[S_ROOT + 2] - 0.5f) - B.measured_heights[(size_t)e * npts + i], -1.0f, 1.0f) * cfg.obs_scale_height;
-  }
+  store_heights_obs(cfg, B, e, 1, v.root, lane, 32);
 }
 
 __global__ void fill_uniform_kernel(float* out, int n, uint64_t seed, uint64_t step) {
@@ -692,7 +263,7 @@ static int post_physics_step(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, c
     return DWBC_ERR_ARG;
   // both kernels move observation rows and history rows in 16-byte vectors
   if (!aligned16(buf->obs_buf) || !aligned16(buf->obs_history)) return DWBC_ERR_UNSUPPORTED;
-  // v2 (16 envs per CTA, TMA bulk copies) whenever the shard is a multiple of 32 envs and every block is 16-B aligned
+  // the TMA kernel (16 envs per CTA, bulk copies) whenever the shard is a multiple of 32 envs and every block is 16-B aligned
   if (cfg->num_envs % 32 == 0 && aligned16(buf->root_states) && aligned16(buf->dof_state) && aligned16(buf->force_sensor) &&
       aligned16(buf->torques) && aligned16(buf->actions) && aligned16(buf->action_history) && aligned16(buf->mass_params) &&
       aligned16(buf->friction) && aligned16(buf->motor_strength) && aligned16(buf->goal_state) && aligned16(buf->derived_state) &&
