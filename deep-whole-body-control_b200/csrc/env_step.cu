@@ -9,7 +9,9 @@
 // this kernel runs everything else.  Both call the per-env functions of env_step_common.cuh on the
 // env's rows staged in shared memory: this kernel runs the warp functions with its warp and
 // scalar_step() on lane 0.  The history row is read as 128-bit streaming loads issued before anything
-// else (so ~86 KB are in flight per SM), re-emitted into obs_buf and shifted in place.
+// else (so ~86 KB are in flight per SM), re-emitted into obs_buf and shifted in place.  With a device
+// step record (a captured step whose step, push decision and curriculum values are read at run time)
+// both kernels build their step arguments in shared memory once per CTA (step_args_to_shared).
 //
 // Compiled with -fmad=false so that discrete decisions (collision rejection, command dead-band,
 // termination thresholds) see the same fp32 roundings as the reference's unfused torch arithmetic.
@@ -36,14 +38,23 @@ static_assert(S_DOF - S_ROOT >= 26 && S_EE - S_DOF >= 2 * DWBC_MAX_DOF && S_GS -
 // 32-float4 chunks: each chunk is loaded, written to obs clipped (WG:992, 1195-1196), and after a __syncwarp written back one num_prop
 // row lower (WG:997-999).  In place is safe: the targets of chunk i lie below its end, so chunks <= i have read them already.
 // The minimum of 1 CTA per SM keeps ptxas from capping the streaming form at 64 registers, where it spills.
-template <bool kLong>
+// kDev = true: a launch of dwbc_post_physics_step_device; each CTA builds its step arguments from Ah and the device record `dev` in
+// shared memory once.  kDev = false reads Ah directly: building the copy cost an eager launch 0.3-0.4 us (H100 SXM, 700 W).
+static_assert(STEP_ARGS_WORDS <= ENV_WARPS * 32, "step_args_to_shared: one word per thread");
+template <bool kLong, bool kDev>
 __global__ void __launch_bounds__(ENV_WARPS * 32, 1)
 env_step_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant__ DwbcEnvBuffers B,
-                const __grid_constant__ DwbcStepArgs A) {
+                const __grid_constant__ DwbcStepArgs Ah, const DwbcStepDevice* __restrict__ dev) {
   __shared__ __align__(16) float smem[ENV_WARPS * S_TOTAL];
+  __shared__ DwbcStepArgs As;
+  const DwbcStepArgs& A = kDev ? As : Ah;     // this step's arguments
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int e = blockIdx.x * ENV_WARPS + wid;
-  if (e >= cfg.num_envs) return;
+  // kDev: the tail CTA of a ragged shard has idle warps; they still write their words of As and reach the barrier below
+  const bool active = e < cfg.num_envs;
+  if constexpr (!kDev) {
+    if (!active) return;
+  }
   float* sm = smem + wid * S_TOTAL;
   const int nd = cfg.num_dofs, na = cfg.num_actions, ahl = cfg.action_hist_len, P = cfg.num_prop, H = cfg.history_len;
   const int nbp1 = cfg.num_bodies_p1;
@@ -57,8 +68,13 @@ env_step_kernel(const __grid_constant__ DwbcEnvCfg cfg, const __grid_constant__ 
 #pragma unroll
     for (int i = 0; i < MAX_H4; ++i) {
       int idx = lane + 32 * i;
-      h[i] = idx < nh4 ? ldg_stream(hist4 + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
+      h[i] = active && idx < nh4 ? ldg_stream(hist4 + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
+  }
+  if constexpr (kDev) {
+    step_args_to_shared(Ah, dev, &As, threadIdx.x);
+    __syncthreads();
+    if (!active) return;
   }
   // ---- 2. coalesced staging of the env's rows ----------------------------------------------------
   float* root_g = B.root_states + (size_t)e * 26;
@@ -210,6 +226,18 @@ int dwbc_launch_env_step_v2(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, co
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
+// The kernels read a device step record from device memory: device or managed memory, or host memory registered with CUDA and mapped at
+// the same address.  A pointer the runtime does not know as one of these (plain host memory, a stale address), or a failed query, is
+// refused before anything is launched instead of faulting in the kernel.  Only calls with a record (captures) pay for the query.
+static bool device_readable(const void* p) {
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    (void)cudaGetLastError();   // not sticky: clear it so that the next launch check does not report it
+    return false;
+  }
+  return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged || (a.type == cudaMemoryTypeHost && a.devicePointer == p);
+}
+
 // extras['episode'] of one step in a fixed order: block c adds column c of the slots of the envs that reset, in env order (thread t:
 // envs t, t + 256, ...; then a fixed tree), column 0 counting them; episode_stats[c] += that sum
 // With a device step record (dwbc_post_physics_step_device) block 0 also advances its step: the post-physics kernel before it has used it.
@@ -263,6 +291,7 @@ static int post_physics_step(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, c
     return DWBC_ERR_ARG;
   // both kernels move observation rows and history rows in 16-byte vectors
   if (!aligned16(buf->obs_buf) || !aligned16(buf->obs_history)) return DWBC_ERR_UNSUPPORTED;
+  if (dev && !device_readable(dev)) return DWBC_ERR_UNSUPPORTED;
   // the TMA kernel (16 envs per CTA, bulk copies) whenever the shard is a multiple of 32 envs and every block is 16-B aligned
   if (cfg->num_envs % 32 == 0 && aligned16(buf->root_states) && aligned16(buf->dof_state) && aligned16(buf->force_sensor) &&
       aligned16(buf->torques) && aligned16(buf->actions) && aligned16(buf->action_history) && aligned16(buf->mass_params) &&
@@ -271,14 +300,13 @@ static int post_physics_step(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, c
     const int rc = dwbc_launch_env_step_v2(cfg, buf, args, dev, (cudaStream_t)stream);
     if (rc != DWBC_ERR_UNSUPPORTED) return rc == DWBC_OK ? launch_episode_stats(cfg, buf, dev, (cudaStream_t)stream) : rc;
   }
-  if (dev) return DWBC_ERR_UNSUPPORTED;      // the warp-per-env kernel reads the host fields only
   const int grid = (cfg->num_envs + ENV_WARPS - 1) / ENV_WARPS;
-  if ((int64_t)cfg->history_len * cfg->num_prop <= MAX_H4 * 128)
-    env_step_kernel<false><<<grid, ENV_WARPS * 32, 0, (cudaStream_t)stream>>>(*cfg, *buf, *args);
-  else
-    env_step_kernel<true><<<grid, ENV_WARPS * 32, 0, (cudaStream_t)stream>>>(*cfg, *buf, *args);
+  const bool long_row = (int64_t)cfg->history_len * cfg->num_prop > MAX_H4 * 128;
+  auto kern = long_row ? (dev ? env_step_kernel<true, true> : env_step_kernel<true, false>)
+                       : (dev ? env_step_kernel<false, true> : env_step_kernel<false, false>);
+  kern<<<grid, ENV_WARPS * 32, 0, (cudaStream_t)stream>>>(*cfg, *buf, *args, dev);
   DWBC_LAUNCH_CHECK();
-  return launch_episode_stats(cfg, buf, nullptr, (cudaStream_t)stream);
+  return launch_episode_stats(cfg, buf, dev, (cudaStream_t)stream);
 }
 
 extern "C" int dwbc_post_physics_step(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, const DwbcStepArgs* args,

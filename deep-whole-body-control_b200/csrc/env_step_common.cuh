@@ -14,6 +14,28 @@ enum { F_RESET = 1, F_TIMEOUT = 2, F_FILL = 4, F_OOB = 8, F_ROOT_DIRTY = 16, F_D
 enum { FE_ENERGY_SQ = 0, FE_LEG_ABS, FE_LEG_SUM, FE_ARM_ABS, FE_TORQUE_SQ, FE_DOFVEL_SQ, FE_DOF_ACC, FE_ACT_RATE, FE_HIP_L2, FE_LEG_L2,
        FE_FOOT_Z, FE_POS_LIM, FE_VEL_LIM, FE_TQ_LIM, FE_STAND, FE_COUNT = 16 };
 
+// Word `tid` of the step arguments a kernel works with: the host's DwbcStepArgs, except that with a device record (CUDA-graph replay) the
+// step, the push decision (WG:934) and the curriculum values come from that record.  Threads 0 .. STEP_ARGS_WORDS - 1 take part; each
+// kernel asserts that its CTA has that many threads.
+static_assert(offsetof(DwbcStepArgs, generic_kernel) - offsetof(DwbcStepArgs, lin_vel_x) == sizeof(DwbcStepDevice) - offsetof(DwbcStepDevice, lin_vel_x),
+              "the curriculum block of DwbcStepDevice mirrors the one of DwbcStepArgs");
+static_assert(sizeof(DwbcStepArgs) % 4 == 0, "one word per thread");
+constexpr int STEP_ARGS_WORDS = sizeof(DwbcStepArgs) / 4;
+__device__ __forceinline__ void step_args_to_shared(const DwbcStepArgs& h, const DwbcStepDevice* d, DwbcStepArgs* out, int tid) {
+  constexpr int W_STEP = offsetof(DwbcStepArgs, step) / 4, W_PUSH = offsetof(DwbcStepArgs, do_push) / 4;
+  constexpr int W_CUR0 = offsetof(DwbcStepArgs, lin_vel_x) / 4, W_CUR1 = offsetof(DwbcStepArgs, generic_kernel) / 4;
+  if (tid >= STEP_ARGS_WORDS) return;
+  uint32_t v = reinterpret_cast<const uint32_t*>(&h)[tid];
+  if (d) {
+    const uint64_t step = d->step;
+    if (tid >= W_CUR0 && tid < W_CUR1) v = reinterpret_cast<const uint32_t*>(d->lin_vel_x)[tid - W_CUR0];
+    else if (tid == W_STEP) v = (uint32_t)step;
+    else if (tid == W_STEP + 1) v = (uint32_t)(step >> 32);
+    else if (tid == W_PUSH) v = (d->push_interval > 0 && step % (uint64_t)d->push_interval == 0) ? 1u : 0u;
+  }
+  reinterpret_cast<uint32_t*>(out)[tid] = v;
+}
+
 // One env's staged rows (shared memory).
 struct EnvView {
   float* root;         // [26] root state: base 0..12, box 13..15

@@ -94,25 +94,7 @@ struct V2 {
                     NPRIV % 4 == 0, "TMA blocks must be multiples of 16 bytes");
 };
 
-// Word `tid` of the step arguments a kernel works with: the host's DwbcStepArgs, except that with a device record (CUDA-graph replay) the
-// step, the push decision (WG:934) and the curriculum values come from that record.  Threads 0 .. sizeof(DwbcStepArgs) / 4 - 1 take part.
-static_assert(offsetof(DwbcStepArgs, generic_kernel) - offsetof(DwbcStepArgs, lin_vel_x) == sizeof(DwbcStepDevice) - offsetof(DwbcStepDevice, lin_vel_x),
-              "the curriculum block of DwbcStepDevice mirrors the one of DwbcStepArgs");
-static_assert(sizeof(DwbcStepArgs) / 4 <= V2_THREADS && sizeof(DwbcStepArgs) % 4 == 0, "one word per thread");
-__device__ __forceinline__ void step_args_to_shared(const DwbcStepArgs& h, const DwbcStepDevice* d, DwbcStepArgs* out, int tid) {
-  constexpr int NW = sizeof(DwbcStepArgs) / 4, W_STEP = offsetof(DwbcStepArgs, step) / 4, W_PUSH = offsetof(DwbcStepArgs, do_push) / 4;
-  constexpr int W_CUR0 = offsetof(DwbcStepArgs, lin_vel_x) / 4, W_CUR1 = offsetof(DwbcStepArgs, generic_kernel) / 4;
-  if (tid >= NW) return;
-  uint32_t v = reinterpret_cast<const uint32_t*>(&h)[tid];
-  if (d) {
-    const uint64_t step = d->step;
-    if (tid >= W_CUR0 && tid < W_CUR1) v = reinterpret_cast<const uint32_t*>(d->lin_vel_x)[tid - W_CUR0];
-    else if (tid == W_STEP) v = (uint32_t)step;
-    else if (tid == W_STEP + 1) v = (uint32_t)(step >> 32);
-    else if (tid == W_PUSH) v = (d->push_interval > 0 && step % (uint64_t)d->push_interval == 0) ? 1u : 0u;
-  }
-  reinterpret_cast<uint32_t*>(out)[tid] = v;
-}
+static_assert(STEP_ARGS_WORDS <= V2_THREADS, "step_args_to_shared: one word per thread");
 
 template <int ND, int NA, int AH, int P, int H, int NPRIV>
 __global__ void __launch_bounds__(V2_THREADS, 2)

@@ -219,8 +219,10 @@ int dwbc_post_physics_step(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, con
 
 /* dwbc_post_physics_step whose step, push decision and curriculum values come from the DEVICE record `device` at run time, so that a
  * captured launch stays right on every replay (seed, rand_uniform and generic_kernel stay the host fields of `args`; its step, do_push
- * and curriculum fields are ignored).  The call advances device->step by one in stream order after the kernel has used it.  Only the
- * 16-envs-per-CTA kernel reads a device record: a call that would take the warp-per-env kernel returns DWBC_ERR_UNSUPPORTED. */
+ * and curriculum fields are ignored).  The call advances device->step by one in stream order after the kernel has used it.  Both
+ * kernels read a device record, so every configuration dwbc_post_physics_step accepts is accepted here, with the same results.  The
+ * record must be device-readable memory (device, managed, or registered and mapped host memory): any other pointer is
+ * DWBC_ERR_UNSUPPORTED, before anything is launched. */
 int dwbc_post_physics_step_device(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, const DwbcStepArgs* args, DwbcStepDevice* device,
                                   dwbc_stream_t stream);
 

@@ -1,13 +1,15 @@
 #!/usr/bin/env python
-"""Eager against CUDA-graph replay on bench.py's flat workload (4096 envs, T = 40, tf32x3, 5 epochs x 4 mini-batches).
+"""Eager against CUDA-graph replay on bench.py's flat workload (T = 40, tf32x3, 5 epochs x 4 mini-batches) at --hist history steps and
+--envs envs (default 10 and 4096: bench.py's own workload; built by tools/history_bench.py's workload()).
 
 Two workloads from the same seeds, one eager and one with a captured rollout (dwbc_b200.graphs.RolloutGraph) and captured update()
 (FusedPPO(cuda_graphs=True)), run one iteration each in turn, --runs times (after --warmup iterations each).  Per iteration it records
 the rollout, update() and whole-iteration times (CUDA events), the host CPU time of the process (time.process_time; it includes the time
 the host waits in the iteration's one synchronisation), the host wall time spent enqueueing the rollout, and the library calls made
-through the ctypes binding.  The card's name, power limit and clocks are read in the same run.
+through the ctypes binding.  Which post-physics kernel ran is read from derived_state column 27 (the TMA kernel's out-of-range history
+counter; the warp-per-env kernel leaves it at 0).  The card's name, power limit and clocks are read in the same run.
 
-    python tools/graph_timing.py [--runs 5] [--warmup 3] [--out DIR]
+    python tools/graph_timing.py [--hist 10] [--envs 4096] [--runs 5] [--warmup 3] [--out DIR]
 """
 import argparse
 import json
@@ -15,6 +17,7 @@ import os
 import subprocess
 import sys
 import time
+from types import SimpleNamespace
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -52,12 +55,14 @@ def gpu_info():
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--hist", type=int, default=10, choices=[10, 20, 50], help="history_len (StateHistoryEncoder tsteps)")
+    ap.add_argument("--envs", type=int, default=4096)
     ap.add_argument("--runs", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     assert torch.cuda.is_available(), "graph_timing.py measures on a CUDA device"
-    import bench
+    from history_bench import workload
     from dwbc_b200 import _lib as L
     from dwbc_b200.graphs import RolloutGraph
     counting = CountingLib(L.lib())
@@ -65,10 +70,30 @@ def main():
 
     arms = {}
     for name in ("eager", "graphs"):
-        w = bench.Workload("cuda:0", 0, precision="tf32x3")
-        w.alg.cuda_graphs = name == "graphs"
-        rg = RolloutGraph(w.alg, w.env, physics=lambda t, w=w: w.env.bind_sim(**w.pool[t])) if name == "graphs" else None
+        _, env, alg, pool = workload(args.hist, "tf32x3", args.envs)
+        env.set_obs_target(alg.storage.obs_row(0))
+        w = SimpleNamespace(env=env, alg=alg, pool=pool, obs=alg.storage.obs_row(0), last=None)
+        alg.cuda_graphs = name == "graphs"
+        rg = RolloutGraph(alg, env, physics=lambda t, w=w: w.env.bind_sim(**w.pool[t])) if name == "graphs" else None
         arms[name] = dict(w=w, rg=rg, rows=[])
+
+    def rollout(w):
+        """bench.Workload.rollout: the loop RolloutGraph captures, obs_T of the previous iteration carried into storage row 0."""
+        env, alg, s = w.env, w.alg, w.alg.storage
+        obs = w.obs
+        if obs.data_ptr() != s.obs_row(0).data_ptr():
+            s.obs_row(0).copy_(obs)
+            obs = s.obs_row(0)
+        for t in range(s.num_transitions_per_env):
+            actions = alg.act(obs, obs)
+            env.bind_sim(**w.pool[t])
+            env.set_obs_target(s.obs_row(t + 1))
+            env.set_transition_target(s.values[t], s.rewards[t], s.dones[t], alg.gamma)
+            env.pre_physics_step(actions)
+            env.post_physics_step()
+            obs = env.obs_buf
+            alg.process_env_step(env.rew_buf, env.arm_rew_buf, env.reset_buf, env.extras)
+        return obs
 
     def iteration(arm, record):
         w, rg = arm["w"], arm["rg"]
@@ -77,7 +102,7 @@ def main():
         c0, cpu0 = counting.calls, time.process_time()
         ev[0].record()
         h0 = time.perf_counter()
-        obs = rg.run(w.obs) if rg is not None else w.rollout()
+        obs = rg.run(w.obs) if rg is not None else rollout(w)
         h1 = time.perf_counter()
         ev[1].record()
         w.alg.compute_returns(obs)
@@ -99,8 +124,10 @@ def main():
         for arm in arms.values():
             iteration(arm, True)
     info1 = gpu_info()
-    res = {"workload": "bench.py flat: 4096 envs, T=40, tf32x3, 5 epochs x 4 mini-batches", "runs": args.runs, "warmup": args.warmup,
-           "gpu_before": info0, "gpu_after": info1, "torch": torch.__version__}
+    tma = tuple(bool(arm["w"].env._derived_state[:, 27].any()) for arm in arms.values())
+    res = {"workload": f"bench.py flat: {args.envs} envs, history_len {args.hist}, T=40, tf32x3, 5 epochs x 4 mini-batches",
+           "k1_kernel": {(True, True): "TMA", (False, False): "warp-per-env"}.get(tma, f"differs between the arms: {tma}"),
+           "runs": args.runs, "warmup": args.warmup, "gpu_before": info0, "gpu_after": info1, "torch": torch.__version__}
     for name, arm in arms.items():
         rows = arm["rows"]
         res[name] = {k: dict(median=float(np.median([r[k] for r in rows])), min=float(min(r[k] for r in rows)),

@@ -55,23 +55,24 @@ def events_ms(fn, reps):
     return e0.elapsed_time(e1) / reps
 
 
-def run(H, precision, iters):
+def workload(H, precision, n_envs=N_ENVS):
+    """bench.py's flat workload (same seeds, hyper-parameters and synthetic sim-state pool of T entries) at history_len H and n_envs envs:
+    (params, env core, FusedPPO with its storage, pool)."""
     import envstate as E
-    from dwbc_b200 import _lib as L
     from dwbc_b200 import synth
     from dwbc_b200.actor_critic import FlatActorCritic
     from dwbc_b200.config import WidowGo1Params
     from dwbc_b200.env import FusedWidowGo1Core
     from dwbc_b200.ppo import FusedPPO
     dev = "cuda:0"
-    p = WidowGo1Params(num_envs=N_ENVS, **dict(E.ENV_CONFIGS["flat"], history_len=H))
+    p = WidowGo1Params(num_envs=n_envs, **dict(E.ENV_CONFIGS["flat"], history_len=H))
     st = synth.initial_env_state(p, 100)
     st.update(synth.sim_state(p, 100, 0, rp_sigma=0.05, z_lo=0.327))
     env = FusedWidowGo1Core(p, dev, state=st, seed=1000, sync_stats=False)
     env.update_command_curriculum()
     ac = FlatActorCritic(device=dev, seed=0, init_std=[[0.8, 1.0, 1.0] * 4 + [1.0] * 6], num_priv=24, num_hist=H, num_prop=76)
     alg = FusedPPO(ac, device=dev, precision=precision, **HP)
-    alg.init_storage(N_ENVS, T, [p.num_obs], [None], [p.num_actions])
+    alg.init_storage(n_envs, T, [p.num_obs], [None], [p.num_actions])
     alg.counter = 1500
     alg.generator = torch.Generator(device=dev)
     alg.generator.manual_seed(7)
@@ -85,6 +86,14 @@ def run(H, precision, iters):
         q = s["root_states"][:, 0, 3:7]
         s["root_states"][:, 0, 3:7] = q / q.norm(dim=-1, keepdim=True)
         pool.append(s)
+    return p, env, alg, pool
+
+
+def run(H, precision, iters):
+    from dwbc_b200 import _lib as L
+    p, env, alg, pool = workload(H, precision)
+    ac = alg.actor_critic
+    dev = "cuda:0"
     s_ = alg.storage
 
     def rollout():
