@@ -19,6 +19,18 @@ import torch
 from . import _lib as L
 from .config import METRIC_NAMES, RAND_COLS, TERM_ID, CommandCurriculum, WidowGo1Params
 
+CHECKPOINT_VERSION = 1          # layout of FusedWidowGo1Core.state_dict()
+# the task state a checkpoint holds, by checkpoint name (load_state's where it has one) -> attribute; simulator-owned tensors (bind_sim)
+# are the simulator's to save, and the per-env slots of ended episodes (_stats_scratch) are written before they are read
+_CHECKPOINT = dict(actions="actions", action_history_buf="action_history_buf", goal_state="_goal_state", derived_state="_derived_state",
+                   episode_length_buf="_episode_length", obs_history_buf="_hist", episode_sums="_sums", episode_stats="_stats",
+                   mass_params="mass_params_tensor", friction="friction_coeffs_tensor", motor_strength="motor_strength",
+                   env_origins="env_origins", box_env_origins_delta_y="box_env_origins_delta_y", terrain_levels="terrain_levels",
+                   terrain_types="terrain_types", terrain_origins="terrain_origins", measured_heights="measured_heights",
+                   heights_obs="heights_obs", rew_buf="rew_buf", arm_rew_buf="arm_rew_buf", reset_buf="reset_buf",
+                   time_out_buf="time_out_buf")
+_CURRICULUM_RANGES = ("lin_vel_x_ranges", "ang_vel_yaw_ranges", "goal_ee_l_ranges", "goal_ee_p_ranges", "goal_ee_y_ranges")
+
 
 def make_env_cfg(p: WidowGo1Params, sums_stride: int) -> L.EnvCfg:
     c = L.EnvCfg()
@@ -319,6 +331,65 @@ class FusedWidowGo1Core:
         b.rew_buf, b.arm_rew_buf = P(self.rew_buf), P(self.arm_rew_buf)
         b.reset_buf, b.time_out_buf, b.episode_stats = P(self.reset_buf), P(self.time_out_buf), P(self._stats)
         b.episode_scratch = P(self._stats_scratch)
+
+    # ------------------------------------------------------------------ checkpoint of the task state
+    def _checkpoint_tensors(self) -> Dict[str, torch.Tensor]:
+        t = {k: getattr(self, a) for k, a in _CHECKPOINT.items() if getattr(self, a) is not None}
+        t["obs_buf"] = self.obs_buf[:, :self.num_obs]                   # the current observation, wherever it is targeted
+        return t
+
+    def state_dict(self) -> dict:
+        """Everything this core owns that the post-physics step reads or advances: the packed goal / derived rows (all columns,
+        the TMA kernel's out-of-range history counter included), history, action FIFO, episode lengths, sums and unread statistics,
+        per-env constants, terrain state (and the height field when heights are measured), the current observation and the last
+        step's outputs, `common_step_counter`, `seed` and the command curriculum.  The simulator's tensors are not included."""
+        cur = self.curriculum
+        t = {k: v.clone() for k, v in self._checkpoint_tensors().items()}
+        if self.p.measure_heights and self.height_samples is not None:
+            t["height_samples"] = self.height_samples.clone()
+        return dict(version=CHECKPOINT_VERSION, cfg=torch.frombuffer(bytearray(bytes(self._cfg)), dtype=torch.uint8), tensors=t,
+                    common_step_counter=self.common_step_counter, seed=self.seed,
+                    curriculum=dict(update_counter=cur.update_counter, **{k: [float(x) for x in getattr(cur, k)] for k in _CURRICULUM_RANGES},
+                                    reward_scales={k: float(v) for k, v in cur.reward_scales.items()},
+                                    arm_reward_scales={k: float(v) for k, v in cur.arm_reward_scales.items()}))
+
+    def load_state_dict(self, sd: dict):
+        """Restore a state_dict() in place.  A checkpoint of a core built with another DwbcEnvCfg (envs, history length, reward
+        terms, sums layout, ...) or of another format version raises DwbcError before anything is copied.  No tensor is re-bound,
+        except a height field on a core that has none yet: it is allocated and bound as `load_state` does (a captured rollout then
+        re-captures)."""
+        keys = {"version", "cfg", "tensors", "common_step_counter", "seed", "curriculum"}
+        if not isinstance(sd, dict) or sd.get("version") != CHECKPOINT_VERSION or set(sd) != keys:
+            raise L.DwbcError(f"not a FusedWidowGo1Core checkpoint of format version {CHECKPOINT_VERSION}: "
+                              f"version {sd.get('version') if isinstance(sd, dict) else None}")
+        if bytes(sd["cfg"].cpu().numpy()) != bytes(self._cfg):
+            raise L.DwbcError("the checkpoint was taken on a core built with another DwbcEnvCfg (envs, history, reward terms, sums layout, ...)")
+        src, own = sd["tensors"], self._checkpoint_tensors()
+        hs = src.get("height_samples")
+        if set(src) - {"height_samples"} != set(own) or (hs is not None and not self.p.measure_heights):
+            raise L.DwbcError(f"the checkpoint holds the tensors {sorted(src)}, this core {sorted(own)}")
+        for k, dst in own.items():
+            if src[k].shape != dst.shape or src[k].dtype != dst.dtype:
+                raise L.DwbcError(f"{k}: {src[k].dtype}{list(src[k].shape)} in the checkpoint, {dst.dtype}{list(dst.shape)} in this core")
+        if hs is not None and (hs.dtype != torch.int16 or tuple(hs.shape) != (self.p.tot_rows, self.p.tot_cols)):
+            raise L.DwbcError(f"height_samples: {hs.dtype}{list(hs.shape)}, not int16[{self.p.tot_rows}, {self.p.tot_cols}]")
+        cur, c = self.curriculum, sd["curriculum"]
+        if set(c["reward_scales"]) != set(cur.reward_scales) or set(c["arm_reward_scales"]) != set(cur.arm_reward_scales):
+            raise L.DwbcError("the checkpoint's curriculum scales other reward terms")
+        for k, dst in own.items():
+            dst.copy_(src[k])
+        if hs is not None:
+            if self.height_samples is None or self.height_samples.shape != hs.shape:
+                self.height_samples = hs.to(self.device, copy=True).contiguous()
+                self._bind()
+            else:
+                self.height_samples.copy_(hs)
+        self.common_step_counter, self.seed = int(sd["common_step_counter"]), int(sd["seed"])
+        cur.update_counter = int(c["update_counter"])
+        for k in _CURRICULUM_RANGES:
+            setattr(cur, k, np.array(c[k], dtype=np.float64))
+        cur.reward_scales, cur.arm_reward_scales = dict(c["reward_scales"]), dict(c["arm_reward_scales"])
+        self._refresh_args()
 
     # ------------------------------------------------------------------ curriculum (WG:678-692)
     def update_command_curriculum(self):

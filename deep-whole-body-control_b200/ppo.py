@@ -25,6 +25,8 @@ from .actor_critic import FlatActorCritic
 from .graphs import HostUpload
 from .storage import FusedRolloutStorage
 
+CHECKPOINT_VERSION = 1          # layout of FusedPPO.state_dict()
+
 
 class _AdamState:
     """Flat Adam state of one parameter group; `state_dict()` mimics torch.optim.Adam's layout."""
@@ -36,15 +38,35 @@ class _AdamState:
         self.step = 0
         self.param_groups = [dict(lr=lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=0)]
 
+    def _names(self):
+        return [n for n in self.ac.offsets if self.first <= self.ac.offsets[n] < self.first + self.count]
+
+    def check_state_dict(self, sd, what):
+        """Raise DwbcError unless `sd` is a state_dict() of this group: one entry per parameter, the parameters' shapes, one step."""
+        names, shapes = self._names(), dict(self.ac.manifest)
+        try:
+            params, state = list(sd["param_groups"][0]["params"]), sd["state"]
+            if params != list(range(len(names))) or (state and set(state) != set(params)):
+                raise L.DwbcError(f"{what}: {len(params)} parameters in the checkpoint, {len(names)} in this optimizer")
+            for i, n in enumerate(names):
+                if i in state:
+                    st = state[i]
+                    if tuple(st["exp_avg"].shape) != shapes[n] or tuple(st["exp_avg_sq"].shape) != shapes[n]:
+                        raise L.DwbcError(f"{what}: the moments of {n} have shape {tuple(st['exp_avg'].shape)}, not {shapes[n]}")
+            if len({int(st["step"]) for st in state.values()}) > 1:
+                raise L.DwbcError(f"{what}: the parameters have different step counts")
+        except (KeyError, IndexError, TypeError, AttributeError) as e:
+            raise L.DwbcError(f"{what}: not an optimizer state_dict ({type(e).__name__}: {e})") from None
+
     def state_dict(self):
-        names = [n for n in self.ac.offsets if self.first <= self.ac.offsets[n] < self.first + self.count]
+        names = self._names()
         um, uv = self.ac.unflat(self.m), self.ac.unflat(self.v)
         state = {i: dict(step=torch.tensor(float(self.step)), exp_avg=um[n].clone(), exp_avg_sq=uv[n].clone())
                  for i, n in enumerate(names)} if self.step > 0 else {}
         return dict(state=state, param_groups=[dict(self.param_groups[0], params=list(range(len(names))))])
 
     def load_state_dict(self, sd):
-        names = [n for n in self.ac.offsets if self.first <= self.ac.offsets[n] < self.first + self.count]
+        names = self._names()
         um, uv = self.ac.unflat(self.m), self.ac.unflat(self.v)
         for i, n in enumerate(names):
             if i in sd["state"]:
@@ -468,3 +490,64 @@ class FusedPPO:
         self._packed = False
         L.check(self._lib.dwbc_enforce_min_std(L.ptr(ac.flat), ac.offsets["std"], L.ptr(self.min_policy_std),
                                                self.min_policy_std.numel(), L.stream_ptr()), "dwbc_enforce_min_std")
+
+    # ------------------------------------------------------------------ checkpoint of the training state
+    def _rng(self):
+        """The generator `act` and `draw_indices` draw from: `generator`, or the device's default generator when it is None."""
+        if self.generator is not None:
+            return self.generator
+        if self.device.type == "cuda":
+            return torch.cuda.default_generators[self.device.index if self.device.index is not None else torch.cuda.current_device()]
+        return torch.default_generator
+
+    def _storage_shape(self):
+        s = self.storage
+        return None if s is None else (s.num_envs, s.num_transitions_per_env, tuple(s.obs_shape), tuple(s.actions_shape))
+
+    def state_dict(self):
+        """Everything later iterations depend on: parameters (reference names), both Adam states, `counter` (the schedules) and the
+        generator state.  Precision and hyper-parameters are constructor choices and are not saved.  Taken between iterations only:
+        a rollout in progress (storage.step != 0) raises DwbcError."""
+        if self.storage is not None and self.storage.step != 0:
+            raise L.DwbcError(f"state_dict() between iterations only: the storage holds {self.storage.step} steps of a rollout")
+        return dict(version=CHECKPOINT_VERSION, actor_critic=self.actor_critic.state_dict(), optimizer=self.optimizer.state_dict(),
+                    hist_encoder_optimizer=self.hist_encoder_optimizer.state_dict(), counter=self.counter,
+                    generator=self._rng().get_state(), storage=self._storage_shape())
+
+    def load_state_dict(self, sd):
+        """Restore a state_dict() in place, so that the next iteration computes what it computed after the save.  Everything is
+        checked first (format version, parameter names and shapes, storage shape, both optimizer states, generator state); a refused
+        load raises DwbcError and changes nothing.  No tensor is re-bound, so captured graphs stay valid."""
+        keys = {"version", "actor_critic", "optimizer", "hist_encoder_optimizer", "counter", "generator", "storage"}
+        if not isinstance(sd, dict) or sd.get("version") != CHECKPOINT_VERSION or set(sd) != keys:
+            raise L.DwbcError(f"not a FusedPPO checkpoint of format version {CHECKPOINT_VERSION}: "
+                              f"version {sd.get('version') if isinstance(sd, dict) else None}")
+        ac, params = self.actor_critic, sd["actor_critic"]
+        if set(params) != set(ac.views):
+            raise L.DwbcError(f"the checkpoint's network has other parameters: missing {[n for n in ac.views if n not in params]}, "
+                              f"unexpected {[n for n in params if n not in ac.views]}")
+        for n, shape in ac.manifest:
+            if tuple(params[n].shape) != shape:
+                raise L.DwbcError(f"parameter {n} has shape {tuple(params[n].shape)} in the checkpoint, {shape} in this network")
+        if sd["storage"] != self._storage_shape():
+            raise L.DwbcError(f"the checkpoint was taken with storage (envs, steps, obs, actions) {sd['storage']}, this one is "
+                              f"{self._storage_shape()}")
+        self.optimizer.check_state_dict(sd["optimizer"], "optimizer")
+        self.hist_encoder_optimizer.check_state_dict(sd["hist_encoder_optimizer"], "hist_encoder_optimizer")
+        rng, gen = self._rng(), sd["generator"]
+        cur = rng.get_state()
+        if not isinstance(gen, torch.Tensor) or gen.dtype != cur.dtype or gen.shape != cur.shape:
+            raise L.DwbcError(f"the checkpoint's generator state does not fit the {rng.device} generator of this algorithm")
+        if not isinstance(sd["counter"], int) or sd["counter"] < 0:
+            raise L.DwbcError(f"counter {sd['counter']!r} is not an iteration count")
+        ac.load_state_dict(params)
+        for opt, key in ((self.optimizer, "optimizer"), (self.hist_encoder_optimizer, "hist_encoder_optimizer")):
+            opt.m.zero_()
+            opt.v.zero_()
+            opt.step = 0
+            opt.load_state_dict(sd[key])
+        self.counter = sd["counter"]
+        rng.set_state(gen)
+        if self.storage is not None:
+            self.storage.clear()             # the checkpoint was taken between iterations
+        self.params_changed()
