@@ -244,7 +244,8 @@ def minibatch_loss(P, mb, hp, counter):
         vloss = (mb["returns"] - value).pow(2).mean()
     creg = priv_reg_coef(counter, hp["priv_reg_coef_schedual"])
     loss = surr + hp["value_loss_coef"] * vloss - hp["entropy_coef"] * ent.mean() + creg * reg
-    info = dict(surrogate=surr.detach(), value=vloss.detach(), priv_reg=reg.detach(), priv_reg_coef=creg, mixing_ratio=rho)
+    info = dict(surrogate=surr.detach(), value=vloss.detach(), priv_reg=reg.detach(), entropy=ent.mean().detach(), priv_reg_coef=creg,
+                mixing_ratio=rho)
     if hp.get("torque_supervision", False):
         assert not hp.get("adaptive_arm_gains", False), "only the fixed-gain branch (PPO:229-231, 318-323) is restated"
         n_arm = mb["target_arm_torques"].shape[-1]

@@ -50,8 +50,15 @@ def test_gae_matches_reference_golden():
     np.testing.assert_allclose(alg.storage.advantages.cpu().numpy(), g["advantages"], rtol=1e-5, atol=2e-6)
 
 
-@pytest.mark.parametrize("N,T", [(4096, 40), (8192, 24), (37, 5)])
-def test_gae_matches_oracle_full_size(N, T):
+@pytest.mark.parametrize("N,T,gamma,lam", [
+    pytest.param(4096, 40, 0.99, 0.95, id="4096-40"), pytest.param(8192, 24, 0.99, 0.95, id="8192-24"),
+    pytest.param(37, 5, 0.99, 0.95, id="37-5"),
+    pytest.param(40000, 8, 0.99, 0.95, id="40000-8"),                     # more columns than DWBC_GAE_MAX_BLOCKS x 64: the blocks loop
+    pytest.param(4096, 40, 0.998, 0.95, id="4096-40-gamma0.998"),          # FusedPPO's default gamma
+    pytest.param(4096, 40, 0.99, 1.0, id="4096-40-lam1"), pytest.param(4096, 40, 0.99, 0.0, id="4096-40-lam0"),
+    pytest.param(37, 1, 0.99, 0.95, id="37-1"),                            # a one-step rollout
+])
+def test_gae_matches_oracle_full_size(N, T, gamma, lam):
     from dwbc_b200.storage import FusedRolloutStorage
     s = FusedRolloutStorage(N, T, [8], [None], [18], "cuda:0")
     rew = torch.from_numpy(synth.normal(1, 1, (T, N, 2)))
@@ -59,8 +66,8 @@ def test_gae_matches_oracle_full_size(N, T):
     dones = torch.from_numpy(synth.bernoulli(1, 3, (T, N, 1), 0.05)).to(torch.uint8)
     last = torch.from_numpy(synth.normal(1, 4, (N, 2)))
     s.rewards.copy_(rew.cuda()); s.values.copy_(val.cuda()); s.dones.copy_(dones.cuda())
-    s.compute_returns(last.cuda(), 0.99, 0.95)
-    ret, adv = PO.compute_returns(rew, val, dones, last, 0.99, 0.95)
+    s.compute_returns(last.cuda(), gamma, lam)
+    ret, adv = PO.compute_returns(rew, val, dones, last, gamma, lam)
     np.testing.assert_allclose(s.returns.cpu().numpy(), ret.numpy(), rtol=1e-6, atol=1e-6)
     np.testing.assert_allclose(s.advantages.cpu().numpy(), adv.numpy(), rtol=1e-5, atol=2e-6)
     a = s.advantages.double()
@@ -69,7 +76,7 @@ def test_gae_matches_oracle_full_size(N, T):
     from dwbc_b200 import _lib as L
     s.advantages.zero_(); s._stats.zero_()
     L.check(L.lib().dwbc_gae(L.ptr(s.rewards), L.ptr(s.values), L.ptr(s.dones), L.ptr(last.cuda()), L.ptr(s.returns),
-                             L.ptr(s.advantages), L.ptr(s._stats), T, N, 0.99, 0.95, 0, L.stream_ptr()), "gae")
+                             L.ptr(s.advantages), L.ptr(s._stats), T, N, gamma, lam, 0, L.stream_ptr()), "gae")
     raw = (ret - val)
     np.testing.assert_allclose(s.advantages.cpu().numpy(), raw.numpy(), rtol=1e-6, atol=1e-6)
     assert float(s._stats[0]) == T * N * 2
