@@ -390,7 +390,7 @@ static __device__ void coop_resample_goal(const DwbcEnvCfg& cfg, const DwbcStepA
   // per round, one (try, path sample) pair per lane, and the lowest passing try wins: same result, 4 rounds instead of 10 in
   // the worst case (the slowest CTA of the launch sets the kernel time).
   V3 goal = start;
-  const int ns = cfg.n_collision_samples > 0 ? (cfg.n_collision_samples < 32 ? cfg.n_collision_samples : 32) : 1;
+  const int ns = cfg.n_collision_samples > 0 ? (cfg.n_collision_samples < 16 ? cfg.n_collision_samples : 16) : 1;   // collision_t[16]
   const int tpr = 32 / ns;                                   // tries per round
   const int my_t = lane / ns, my_s = lane - my_t * ns;       // lane -> (try within the round, path sample)
   bool done = false;
@@ -410,7 +410,7 @@ static __device__ void coop_resample_goal(const DwbcEnvCfg& cfg, const DwbcStepA
     const unsigned hits = __ballot_sync(FULL, hit);
     int win = -1, last = 0;
     for (int t = 0; t < tpr && k0 + t < cfg.max_goal_tries; ++t) {
-      const unsigned m = (ns == 32 ? FULL : ((1u << ns) - 1u)) << (t * ns);
+      const unsigned m = ((1u << ns) - 1u) << (t * ns);
       last = t;
       if (win < 0 && (hits & m) == 0) win = t;
     }

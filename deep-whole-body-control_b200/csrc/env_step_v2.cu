@@ -294,7 +294,7 @@ using namespace dwbc;
 int dwbc_launch_env_step_v2(const DwbcEnvCfg* cfg, const DwbcEnvBuffers* buf, const DwbcStepArgs* args, const DwbcStepDevice* dev, cudaStream_t st) {
   using K = V2<20, 18, 4, 76, 10, 24>;
   if (cfg->num_dofs != 20 || cfg->num_actions != 18 || cfg->action_hist_len != 4 || cfg->num_prop != 76 || cfg->history_len != 10 ||
-      cfg->num_priv != 24 || (cfg->sums_stride & 3) || cfg->n_collision_samples > 32)
+      cfg->num_priv != 24 || (cfg->sums_stride & 3) || cfg->n_collision_samples > 16)
     return DWBC_ERR_UNSUPPORTED;
   const size_t smem = (size_t)(K::o_sums + V2_E * cfg->sums_stride) * sizeof(float);
   if (smem > 110 * 1024) return DWBC_ERR_UNSUPPORTED;      // two CTAs per SM

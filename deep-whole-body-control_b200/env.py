@@ -56,6 +56,9 @@ def make_env_cfg(p: WidowGo1Params, sums_stride: int) -> L.EnvCfg:
     c.goal_is_cart = int(p.command_mode == "cart")
     c.max_episode_length = int(p.max_episode_length)
     c.resample_interval = p.resample_interval
+    if not 0 <= p.num_collision_check_samples <= len(c.collision_t):
+        raise L.DwbcError(f"num_collision_check_samples = {p.num_collision_check_samples}: the kernels take 0 .. {len(c.collision_t)} "
+                          f"collision samples per path")
     c.n_collision_samples, c.max_goal_tries = p.num_collision_check_samples, 10
     c.only_positive_rewards = int(p.only_positive_rewards)
     slots = p.sum_slots()

@@ -13,6 +13,7 @@ if ROOT not in sys.path:
 import dwbc_b200  # noqa: E402,F401
 from dwbc_b200 import synth  # noqa: E402
 
+_DEFAULT_DOF_POS = dwbc_b200.WidowGo1Params().default_dof_pos     # repeated per leg: [0.1, 0.8, -1.5] with the hip sign alternating
 ENV_CONFIGS = {
     # default widowGo1 flat config (BASELINE.json configs[1] semantics)
     "flat": dict(),
@@ -34,7 +35,55 @@ ENV_CONFIGS = {
         arm_reward_scales={
             "arm_energy_abs_sum": -0.004, "termination": -1.0, "tracking_ee_cart": 0.3, "tracking_ee_orn": 0.1,
             "tracking_ee_orn_ry": 0.1, "tracking_ee_sphere": 0.55}),
+    # The configs below each set the fields of one branch no shipped config takes (the kernels read them from DwbcEnvCfg / the device
+    # step record); everything else stays at the defaults of `flat`.
+    # cart goals (WG:1360-1366, command_mode): termination signs and observation goal columns read the cart goal; non-zero orientation
+    # deltas whose yaw part d + yaw leaves (-pi, pi], so the wrap of the goal orientation runs (WG:1307-1313)
+    "cart": dict(
+        command_mode="cart", final_delta_orn=[[-0.6, 0.6], [-0.4, 0.8], [-2.6, 2.6]],
+        arm_reward_scales={"arm_energy_abs_sum": -0.004, "tracking_ee_cart": 0.55, "tracking_ee_orn": 0.1, "tracking_ee_orn_ry": 0.1}),
+    # only_positive_rewards and termination on both channels (WG:170-205): mostly negative leg scales, so the channel sum is often
+    # clipped before the termination term is added; the shared `termination` sum slot takes both channels' additions
+    "positive": dict(
+        only_positive_rewards=True,
+        reward_scales={"energy_square": -6e-5, "foot_contacts_z": -1e-4, "hip_action_l2": -0.02, "survive": 0.05, "termination": -2.0,
+                       "torques": -1e-4, "dof_vel": -2e-3, "tracking_ang_vel_yaw_exp": 0.15, "tracking_lin_vel_x_l1": 0.5},
+        arm_reward_scales={"arm_energy_abs_sum": -0.004, "termination": -1.0, "tracking_ee_sphere": 0.55}),
+    # EE-goal search (WG:1316-1342): a collision box and an underground limit that reject most paths, so the winning try takes every
+    # index 0..9 and some searches use up all ten tries; num_collision_check_samples is set per case (goals_case)
+    "goals": dict(underground_limit=-0.1, collision_upper_limits=[0.45, 0.3, 0.1], collision_lower_limits=[-0.3, -0.3, -0.6]),
+    # no DOF reordering (WG:1003-1048) and no push (WG:804-814, 934); 8 penalised and 3 termination contact bodies; per-joint distinct
+    # defaults and limits, read by the reset, the observation and the DOF reward terms
+    "raw": dict(
+        reorder_dofs=False, push_robots=False,
+        penalized_contact_indices=[1, 2, 3, 4, 6, 7, 8, 10], termination_contact_indices=[11, 14, 19],
+        default_dof_pos=[round(d + 0.013 * (i + 1), 3) for i, d in enumerate(_DEFAULT_DOF_POS)],
+        dof_pos_limits=[[round(d + 0.013 * (i + 1) - 0.3 - 0.02 * i, 3), round(d + 0.013 * (i + 1) + 0.25 + 0.015 * i, 3)]
+                        for i, d in enumerate(_DEFAULT_DOF_POS)],
+        dof_vel_limits=[round(1.0 + 0.17 * i, 3) for i in range(20)],
+        torque_limits=[round(3.0 + 0.9 * i, 3) for i in range(20)], soft_torque_limit=0.85,
+        reward_scales={"collision": -1.0, "dof_pos_limits": -10.0, "dof_vel_limits": -0.1, "energy_square": -6e-5, "foot_contacts_z": -1e-4,
+                       "hip_action_l2": -0.01, "stand_still": -0.1, "survive": 0.2, "termination": -2.0, "torque_limits": -0.01,
+                       "tracking_ang_vel_yaw_exp": 0.15, "tracking_lin_vel_x_l1": 0.5}),
+    # action delay FIFO (WG:1162-1173) with a binding clip_actions; action_delay is set per case (delay_case)
+    "delay": dict(clip_actions=0.5),
 }
+COLLISION_SAMPLES = (0, 1, 3, 10, 11, 16)       # 32 / S tries per round of the kernels' goal search: 32, 32, 10, 3, 2, 2
+ACTION_DELAYS = (0, 1, 6)                        # action_hist_len 2, 3, 8
+
+
+def goals_case(S):
+    return dict(ENV_CONFIGS["goals"], num_collision_check_samples=S)
+
+
+def delay_case(d):
+    return dict(ENV_CONFIGS["delay"], action_delay=d, action_hist_len=d + 2)
+
+
+# every config-branch case by name: the new configs, `goals` once per sample count, `delay` once per delay
+BRANCH_CASES = dict(
+    [(k, ENV_CONFIGS[k]) for k in ("cart", "positive", "raw")] + [(f"goals-{s}", goals_case(s)) for s in COLLISION_SAMPLES] +
+    [(f"delay-{d}", delay_case(d)) for d in ACTION_DELAYS])
 
 
 def make_params(name, num_envs):
@@ -86,7 +135,7 @@ def oracle_state(p, st):
               "last_contacts", "env_origins", "box_env_origins_delta_y", "episode_length_buf", "terrain_levels",
               "terrain_types", "terrain_origins"):
         setattr(s, k, T(st[k]))
-    s.actions = s.action_history_buf[:, -3].clone()
+    s.actions = s.action_history_buf[:, -(p.action_delay + 1)].clone()
     if "height_samples" in st:
         s.height_samples = T(st["height_samples"])
     return s
@@ -101,6 +150,6 @@ def load_sim_into_oracle(o, p, sim):
     s.force_sensor.copy_(torch.from_numpy(sim["force_sensor"]))
     s.torques = torch.from_numpy(sim["torques"]).clone()
     a = torch.from_numpy(sim["policy_actions"])[:, p.raisim2ig(p.num_actions)]
-    a = torch.clip(a, -100.0, 100.0)
-    s.action_history_buf = torch.cat([s.action_history_buf[:, 1:], a[:, None, :]], dim=1)
-    s.actions = s.action_history_buf[:, -3].clone()
+    a = torch.clip(a, -p.clip_actions, p.clip_actions)                                   # WG:1163
+    s.action_history_buf = torch.cat([s.action_history_buf[:, 1:], a[:, None, :]], dim=1)  # WG:1166
+    s.actions = s.action_history_buf[:, -(p.action_delay + 1)].clone()                    # WG:1167-1168

@@ -211,18 +211,20 @@ def test_kernels_agree_on_device_records():
     assert record_step(recs[0]) == record_step(recs[1]) == 141 + steps
 
 
-@pytest.mark.parametrize("H,N", [(50, 1000), (10, 33)], ids=["h50-1000", "h10-33"])
-def test_device_record_equals_host_arguments_on_warp_per_env_kernel(H, N):
+@pytest.mark.parametrize("H,N,push_robots", [(50, 1000, True), (10, 33, True), (10, 33, False)], ids=["h50-1000", "h10-33", "h10-33-no-push"])
+def test_device_record_equals_host_arguments_on_warp_per_env_kernel(H, N, push_robots):
     """Steps 150 (push) and 151 on the warp-per-env kernel: a call whose record holds what the host would pass gives the bits of the
-    host-argument call, and advances record.step by exactly 1."""
+    host-argument call, and advances record.step by exactly 1.  With push_robots off the record's push_interval is 0: nothing is pushed
+    at step 150, so the base velocities of the envs that did not reset are still the simulator's."""
     seed = 61
-    p = WidowGo1Params(num_envs=N, history_len=H)
+    p = WidowGo1Params(num_envs=N, history_len=H, push_robots=push_robots)
     st = E.initial(p, seed)
     host, dev = make_core(p, st, seed=5), make_core(p, st, seed=5)
     host.common_step_counter = dev.common_step_counter = 149
     rec = device_record(dev)
+    assert int(L.StepDevice.from_buffer_copy(bytes(rec.cpu().numpy())).push_interval) == (150 if push_robots else 0)
     spoil_host_args(dev)
-    for t, push in ((1, True), (2, False)):
+    for t, push in ((1, push_robots), (2, False)):
         sim = synth.sim_state(p, seed, t)
         for c in (host, dev):
             load_sim(c, p, sim)
@@ -231,3 +233,6 @@ def test_device_record_equals_host_arguments_on_warp_per_env_kernel(H, N):
         assert record_step(rec) == 150 + t
         assert not bool(host._derived_state[:, OOB_AGE].any()), "the TMA kernel ran"
         assert_bitwise(outputs(host), outputs(dev))
+        kept = ~dev.reset_buf.cpu()
+        moved = ~torch.from_numpy(sim["root_states"][:, 0, 7:9] == dev.root_states[:, 7:9].cpu().numpy()).all(dim=1)
+        assert bool(kept.any()) and bool(moved[kept].any()) == push, f"step {149 + t}: push {push}"

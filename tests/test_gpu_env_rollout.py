@@ -26,7 +26,7 @@ JOINT = 3                 # a leg joint (IG order); the waist joint (num_dofs - 
 
 
 def params(name, N, clip=None):
-    kw = dict(E.ENV_CONFIGS[name])
+    kw = dict(E.ENV_CONFIGS[name] if name in E.ENV_CONFIGS else E.BRANCH_CASES[name])
     if clip is not None:
         kw["clip_observations"] = clip
     return WidowGo1Params(num_envs=N, **kw)
@@ -127,7 +127,7 @@ def check_kernel(core, specialised, age, t):
 # ---------------------------------------------------------------------------------------------- against the oracle
 TASK_STATE = ("commands", "goal_timer", "ee_start_sphere", "ee_goal_sphere", "ee_goal_cart", "curr_ee_goal_sphere", "curr_ee_goal_cart",
               "ee_goal_orn_euler", "base_lin_vel", "base_ang_vel", "base_yaw_quat", "last_root_vel", "last_actions", "last_dof_vel",
-              "feet_air_time")
+              "feet_air_time", "ee_goal_delta_orn_euler")
 
 
 def compare_with_oracle(core, orc, p, t, obs, rew, arew, rst):
@@ -143,6 +143,17 @@ def compare_with_oracle(core, orc, p, t, obs, rew, arew, rst):
     np.testing.assert_allclose(core.obs_history_buf.cpu().numpy(), orc.s.obs_history_buf.numpy(), **FTOL, err_msg=f"history {msg}")
     np.testing.assert_allclose(core._root_states.cpu().numpy(), orc.s.root_states_full.numpy(), **FTOL, err_msg=f"root {msg}")
     np.testing.assert_allclose(core.dof_state.cpu().numpy(), orc.s.dof_state.numpy(), **FTOL, err_msg=f"dof {msg}")
+    np.testing.assert_array_equal(core.action_history_buf.cpu().numpy(), orc.s.action_history_buf.numpy(), err_msg=f"action FIFO {msg}")
+    np.testing.assert_array_equal(core.actions.cpu().numpy(), orc.s.actions.numpy(), err_msg=f"delayed actions {msg}")
+    # episode sums, metric sums and, on reset steps, extras['episode'] (WG:743-750) with the tolerance of the golden test
+    for k, v in orc.s.episode_sums.items():
+        np.testing.assert_allclose(core.episode_sums[k].cpu().numpy(), v.numpy(), rtol=1e-4, atol=1e-6, err_msg=f"episode_sums[{k}] {msg}")
+    for k, v in orc.s.episode_metric_sums.items():
+        np.testing.assert_allclose(core.episode_metric_sums[k].cpu().numpy(), v.numpy(), rtol=1e-4, atol=1e-5, err_msg=f"metric {k} {msg}")
+    if bool(rst.any()):
+        ep = orc.extras["episode"]
+        np.testing.assert_allclose([float(core.extras["episode"][k]) for k in ep], [float(ep[k]) for k in ep], rtol=1e-4, atol=1e-6,
+                                   err_msg=f"extras['episode'] {msg}")
     if p.measure_heights:
         np.testing.assert_allclose(core.measured_heights.cpu().numpy(), orc.measured_heights.numpy(), rtol=1e-6, atol=1e-7)
         np.testing.assert_allclose(core.heights_obs.cpu().numpy(),
@@ -240,11 +251,17 @@ def test_shard_sizes_match_oracle(N, specialised):
 
 
 # ---------------------------------------------------------------------------------------------- the two kernels, production mode
-@pytest.mark.parametrize("name,storage_rows", [("flat", False), ("full", False), ("flat", True)], ids=["flat", "full", "flat-storage-rows"])
+PHILOX_CASES = [("flat", False), ("full", False), ("flat", True)] + \
+    [(name, False) for name in ("cart", "positive", "raw", "goals-0", "goals-3", "goals-11", "goals-16")]
+
+
+@pytest.mark.parametrize("name,storage_rows", PHILOX_CASES, ids=[n + ("-storage-rows" if s else "") for n, s in PHILOX_CASES])
 def test_tma_and_generic_kernel_agree_over_philox_rollout(name, storage_rows):
     """4096 envs, in-kernel Philox draws, 60 steps from common_step_counter 140 (push and command resampling at 150, time-outs),
     injected out-of-range events: every output and state buffer bit for bit (both kernels run the per-env code of
-    env_step_common.cuh), episode sums and extras['episode'] included; only the TMA kernel's out-of-range counter column differs."""
+    env_step_common.cuh), episode sums and extras['episode'] included; only the TMA kernel's out-of-range counter column differs.
+    Also on the config branches the TMA kernel takes (envstate.BRANCH_CASES: cart goals, positive-reward clip, unreordered DOFs with
+    more contact bodies, goal searches with 0 .. 16 collision samples)."""
     seed, N, T = 51, 4096, 60
     p = params(name, N)
     st = E.initial(p, seed)
