@@ -53,12 +53,14 @@ class RolloutGraph:
 
     def key(self, hist_encoding):
         """What a captured rollout depends on: the history-encoder flag, the policy (precision, network, parameters, workspace), the
-        storage, and the env core's configuration and task-state buffers (a new tensor bound there, e.g. by `load_state`, re-captures)."""
+        storage, the env core's configuration and task-state buffers (a new tensor bound there, e.g. by `load_state`, re-captures), and
+        the episode tracker's buffers when FusedPPO(track_episodes=C > 0)."""
         a, s, e = self.alg, self.alg.storage, self.env
         env_bufs = tuple(getattr(e._buf, f) for f, _ in L.EnvBuffers._fields_ if f not in _PER_STEP_FIELDS)
+        tracker = () if a._episodes is None else ((a.track_episodes,) + tuple(v.data_ptr() for v in a._episodes.values()),)
         return (bool(hist_encoding), a.precision, s.num_transitions_per_env, s.num_envs, s._obs_all.data_ptr(), a._ws.data_ptr(),
                 a._ws_rows, a.actor_critic.flat.data_ptr(), bytes(a.actor_critic.net_cfg), a.gamma, bytes(e._cfg), env_bufs,
-                int(e._args.generic_kernel), e.seed)
+                int(e._args.generic_kernel), e.seed) + tracker
 
     def _steps(self, hist_encoding):
         """The launches of one rollout, exactly as an eager loop issues them (bench.Workload.rollout)."""

@@ -5,7 +5,7 @@ attributes `actor_critic`, `storage`, `learning_rate`, `optimizer`, `counter`.
 
 Every numerical step runs in libdwbc kernels; this class only sequences launches:
   act            -> dwbc_policy_act, writing straight into the storage rows (no RS:95-114 copies)
-  process_env_step -> dwbc_store_rewards (time-out bootstrap PPO:133-134)
+  process_env_step -> dwbc_store_rewards (time-out bootstrap PPO:133-134) [+ dwbc_track_episodes, OPR:140-154]
   compute_returns  -> dwbc_critic_values + dwbc_gae
   update         -> per mini-batch: dwbc_ppo_minibatch_grad [+ NCCL all-reduce] + dwbc_clip_adam_step
   update_dagger  -> per mini-batch: dwbc_dagger_minibatch_grad [+ all-reduce] + dwbc_clip_adam_step
@@ -81,7 +81,7 @@ class FusedPPO:
                  use_clipped_value_loss=True, schedule="fixed", desired_kl=0.01, device="cuda:0",
                  mixing_schedule=(0.5, 2000, 4000), torque_supervision=False, torque_supervision_schedule=(0.1, 1000, 1000),
                  adaptive_arm_gains=False, min_policy_std=None, dagger_update_freq=20, priv_reg_coef_schedual=(0, 0, 0, 1),
-                 world_size=1, process_group=None, precision="tf32x3", cuda_graphs=False):
+                 world_size=1, process_group=None, precision="tf32x3", cuda_graphs=False, track_episodes=0):
         if adaptive_arm_gains:
             raise L.DwbcError("adaptive_arm_gains (a 12-output arm head, AC:111-125,214-215; off for widowGo1, WGC:168) is not implemented")
         if schedule != "fixed":
@@ -127,6 +127,12 @@ class FusedPPO:
             raise L.DwbcError("cuda_graphs=True does not capture the multi-GPU all-reduce: use world_size == 1")
         self.cuda_graphs = bool(cuda_graphs)
         self._graphs = {}
+        # track_episodes = C > 0: the runner's per-step bookkeeping (OPR:140-154: running returns and lengths, the last C finished
+        # episodes) runs on the device inside process_env_step; episode_buffers() reads it once per call (DESIGN §11)
+        if isinstance(track_episodes, bool) or not isinstance(track_episodes, int) or track_episodes < 0:
+            raise L.DwbcError(f"track_episodes must be a non-negative int (the number of finished episodes kept), not {track_episodes!r}")
+        self.track_episodes = track_episodes
+        self._episodes = None
 
     # ------------------------------------------------------------------ plumbing
     def init_storage(self, num_envs, num_transitions_per_env, actor_obs_shape, critic_obs_shape, action_shape):
@@ -138,6 +144,9 @@ class FusedPPO:
         self._workspace(max(num_envs, num_envs * num_transitions_per_env // self.num_mini_batches))
         if self.torque_supervision:
             self.storage.enable_torque_supervision(self.actor_critic.num_arm_actions)
+        if self.track_episodes:
+            self._episodes = dict(running=torch.zeros(num_envs, 3, device=self.device), ring=torch.zeros(self.track_episodes, 3, device=self.device),
+                                  pos=torch.zeros(2, dtype=torch.int64, device=self.device))
 
     @property
     def precision(self):
@@ -249,14 +258,22 @@ class FusedPPO:
             raise AssertionError("Rollout buffer overflow")                               # RS:96-97
         t = s.step
         stored = infos.get("dwbc_stored_rows") if isinstance(infos, dict) else None
-        if stored is None or stored != (s.rewards[t].data_ptr(), s.dones[t].data_ptr()):
+        store = stored is None or stored != (s.rewards[t].data_ptr(), s.dones[t].data_ptr())
+        if store or self._episodes is not None:
+            d8 = (dones if dones.dtype in (torch.uint8, torch.bool) else (dones != 0)).contiguous()
+        if store:
             # (else: the post-physics kernel already wrote this step's rewards / dones rows, FusedWidowGo1Core.set_transition_target)
             to = infos.get("time_outs") if isinstance(infos, dict) else None
             to8 = None if to is None else (to if to.dtype in (torch.uint8, torch.bool) else (to != 0)).contiguous()
-            d8 = (dones if dones.dtype in (torch.uint8, torch.bool) else (dones != 0)).contiguous()
             L.check(self._lib.dwbc_store_rewards(L.ptr(rewards.float().contiguous(), torch.float32), L.ptr(arm_rewards.float().contiguous(), torch.float32),
                                                  L.ptr(s.values[t]), L.ptr(to8, (torch.uint8, torch.bool)), L.ptr(d8, (torch.uint8, torch.bool)), self.gamma,
                                                  L.ptr(s.rewards[t]), L.ptr(s.dones[t]), s.num_envs, L.stream_ptr()), "dwbc_store_rewards")
+        if self._episodes is not None:
+            # the un-bootstrapped rewards env.step returned (OPR:147), not the storage row
+            e = self._episodes
+            L.check(self._lib.dwbc_track_episodes(L.ptr(rewards.float().contiguous(), torch.float32), L.ptr(arm_rewards.float().contiguous(), torch.float32),
+                                                  L.ptr(d8, (torch.uint8, torch.bool)), s.num_envs, L.ptr(e["running"]), L.ptr(e["ring"]),
+                                                  L.ptr(e["pos"]), self.track_episodes, L.stream_ptr()), "dwbc_track_episodes")
         if self.torque_supervision and isinstance(infos, dict) and "target_arm_torques" in infos:          # PPO:136-142, RS:108-111
             s.target_arm_torques[t].copy_(infos["target_arm_torques"])
             s.current_arm_dof_pos[t].copy_(infos["current_arm_dof_pos"])
@@ -274,6 +291,23 @@ class FusedPPO:
                                              L.stream_ptr()), "dwbc_critic_values")
         self._packed = False                      # dwbc_critic_values re-packs the critic into the same workspace region
         s.compute_returns(self._last_values, self.gamma, self.lam, self.world_size, self.process_group)
+
+    def episode_buffers(self):
+        """OPR's rewbuffer, arm_rewbuffer and lenbuffer (OPR:140-154, maxlen track_episodes) as Python float lists, oldest first: the
+        episodes finished since tracking began, read with one synchronisation."""
+        if self._episodes is None:
+            raise L.DwbcError("episode_buffers() needs FusedPPO(track_episodes=C > 0) and init_storage()")
+        ring = self._episodes["ring"].to("cpu", non_blocking=True)
+        pos = self._episodes["pos"].to("cpu", non_blocking=True)
+        if self.device.type == "cuda":
+            torch.cuda.current_stream(self.device).synchronize()
+        cap = self.track_episodes
+        n = min(int(pos[1]), cap)
+        rows = ring[(int(pos[0]) - n + torch.arange(n)) % cap]
+        return dict(rewbuffer=rows[:, 0].tolist(), arm_rewbuffer=rows[:, 1].tolist(), lenbuffer=rows[:, 2].tolist())
+
+    def _episodes_shape(self):
+        return None if self._episodes is None else (self._episodes["running"].shape[0], self.track_episodes)
 
     # ------------------------------------------------------------------ schedules (PPO:178-179, 301-302)
     def get_value_mixing_ratio(self):
@@ -510,15 +544,25 @@ class FusedPPO:
         a rollout in progress (storage.step != 0) raises DwbcError."""
         if self.storage is not None and self.storage.step != 0:
             raise L.DwbcError(f"state_dict() between iterations only: the storage holds {self.storage.step} steps of a rollout")
-        return dict(version=CHECKPOINT_VERSION, actor_critic=self.actor_critic.state_dict(), optimizer=self.optimizer.state_dict(),
-                    hist_encoder_optimizer=self.hist_encoder_optimizer.state_dict(), counter=self.counter,
-                    generator=self._rng().get_state(), storage=self._storage_shape())
+        sd = dict(version=CHECKPOINT_VERSION, actor_critic=self.actor_critic.state_dict(), optimizer=self.optimizer.state_dict(),
+                  hist_encoder_optimizer=self.hist_encoder_optimizer.state_dict(), counter=self.counter,
+                  generator=self._rng().get_state(), storage=self._storage_shape())
+        if self.track_episodes:
+            # the episode tracker (track_episodes > 0 only, so that checkpoints without it keep the keys of format version 1)
+            sd["episodes"] = None if self._episodes is None else {k: v.clone() for k, v in self._episodes.items()}
+        return sd
 
     def load_state_dict(self, sd):
         """Restore a state_dict() in place, so that the next iteration computes what it computed after the save.  Everything is
         checked first (format version, parameter names and shapes, storage shape, both optimizer states, generator state); a refused
         load raises DwbcError and changes nothing.  No tensor is re-bound, so captured graphs stay valid."""
         keys = {"version", "actor_critic", "optimizer", "hist_encoder_optimizer", "counter", "generator", "storage"}
+        if isinstance(sd, dict) and "episodes" in sd and not self.track_episodes:
+            raise L.DwbcError("the checkpoint holds an episode tracker: load it into FusedPPO(track_episodes=C > 0)")
+        if self.track_episodes:
+            if not isinstance(sd, dict) or "episodes" not in sd:
+                raise L.DwbcError(f"this FusedPPO tracks episodes (track_episodes={self.track_episodes}): the checkpoint holds no tracker")
+            keys.add("episodes")
         if not isinstance(sd, dict) or sd.get("version") != CHECKPOINT_VERSION or set(sd) != keys:
             raise L.DwbcError(f"not a FusedPPO checkpoint of format version {CHECKPOINT_VERSION}: "
                               f"version {sd.get('version') if isinstance(sd, dict) else None}")
@@ -540,6 +584,8 @@ class FusedPPO:
             raise L.DwbcError(f"the checkpoint's generator state does not fit the {rng.device} generator of this algorithm")
         if not isinstance(sd["counter"], int) or sd["counter"] < 0:
             raise L.DwbcError(f"counter {sd['counter']!r} is not an iteration count")
+        if self.track_episodes:
+            self._check_episodes(sd["episodes"])
         ac.load_state_dict(params)
         for opt, key in ((self.optimizer, "optimizer"), (self.hist_encoder_optimizer, "hist_encoder_optimizer")):
             opt.m.zero_()
@@ -548,6 +594,22 @@ class FusedPPO:
             opt.load_state_dict(sd[key])
         self.counter = sd["counter"]
         rng.set_state(gen)
+        if self._episodes is not None:
+            for k, v in self._episodes.items():
+                v.copy_(sd["episodes"][k])
         if self.storage is not None:
             self.storage.clear()             # the checkpoint was taken between iterations
         self.params_changed()
+
+    def _check_episodes(self, ep):
+        """Raise DwbcError unless `ep` is the tracker of a FusedPPO with this one's env count and track_episodes."""
+        mine = self._episodes_shape()
+        try:
+            theirs = None if ep is None else (ep["running"].shape[0], ep["ring"].shape[0])
+            if theirs != mine:
+                raise L.DwbcError(f"the checkpoint's episode tracker is for (envs, capacity) {theirs}, this one for {mine}")
+            if ep is not None and (set(ep) != set(self._episodes) or any(ep[k].shape != v.shape or ep[k].dtype != v.dtype
+                                                                         for k, v in self._episodes.items())):
+                raise L.DwbcError("the checkpoint's episode tracker is not running [N, 3] fp32, ring [C, 3] fp32, pos [2] int64")
+        except (KeyError, IndexError, TypeError, AttributeError) as e:
+            raise L.DwbcError(f"not an episode tracker ({type(e).__name__}: {e})") from None

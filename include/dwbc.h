@@ -261,6 +261,17 @@ int dwbc_gae(const float* rewards, const float* values, const uint8_t* dones, co
              dwbc_stream_t stream);
 int dwbc_normalize_advantages(float* advantages, const double* stats, int64_t count, dwbc_stream_t stream);
 
+/* OnPolicyRunner.learn's per-step episode bookkeeping (OPR:140-154) on the device, for the un-bootstrapped rewards env.step returned:
+ *   running[n,:] += (rew[n], arm_rew[n], 1);  for every n with dones[n] != 0, in ascending n: append running[n,:] to the ring, then
+ *   running[n,:] = 0.
+ * running [N,3] fp32 (leg return, arm return, length) and ring [C,3] fp32 are caller-owned and start zeroed; ring_pos [2] int64 =
+ * (next slot, total appended) starts at (0, 0).  The ring holds the last min(total, C) episodes, oldest at slot (next - min(total, C))
+ * mod C: the contents of rsl_rl's rewbuffer / lenbuffer deques of maxlen C (arm channel alongside).  A step that finishes more than C
+ * episodes keeps its last C.  dones [N] is uint8 / torch.bool.  One single-CTA launch, fixed order, no atomics: bitwise repeatable
+ * and equal to the fp32 adds of the reference.  NULL pointers, N <= 0 or C <= 0: DWBC_ERR_ARG. */
+int dwbc_track_episodes(const float* rew, const float* arm_rew, const uint8_t* dones, int32_t num_envs, float* running, float* ring,
+                        int64_t* ring_pos, int32_t capacity, dwbc_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------- */
 /* ActorCritic + PPO update                                                                  */
 /* ---------------------------------------------------------------------------------------- */

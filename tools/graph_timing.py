@@ -9,7 +9,12 @@ the host waits in the iteration's one synchronisation), the host wall time spent
 through the ctypes binding.  Which post-physics kernel ran is read from derived_state column 27 (the TMA kernel's out-of-range history
 counter; the warp-per-env kernel leaves it at 0).  The card's name, power limit and clocks are read in the same run.
 
-    python tools/graph_timing.py [--hist 10] [--envs 4096] [--runs 5] [--warmup 3] [--out DIR]
+With --track-episodes C two more arms run FusedPPO(track_episodes=C) (the runner's episode bookkeeping on the device, one
+dwbc_track_episodes launch per env step), eagerly and captured, alternating with the two untracked arms.  The tracker's own time per
+step is then measured with CUDA events around 1000 queued launches on synthetic inputs (2 % dones) at --envs and at 40 000 envs, issued
+eagerly and replayed from a CUDA graph.
+
+    python tools/graph_timing.py [--hist 10] [--envs 4096] [--runs 5] [--warmup 3] [--track-episodes C] [--out DIR]
 """
 import argparse
 import json
@@ -53,12 +58,45 @@ def gpu_info():
         return {"error": str(e)}
 
 
+def tracker_step_us(L, n, cap, launches=1000):
+    """Mean time of one dwbc_track_episodes launch at n envs (us): CUDA events around `launches` queued launches, issued eagerly (which
+    the host's launch rate can bound) and replayed from a CUDA graph."""
+    g = torch.Generator(device="cuda:0")
+    g.manual_seed(3)
+    rew, arm = (torch.randn(n, device="cuda:0", generator=g) for _ in range(2))
+    dones = torch.rand(n, device="cuda:0", generator=g) < 0.02
+    running, ring, pos = torch.zeros(n, 3, device="cuda:0"), torch.zeros(cap, 3, device="cuda:0"), torch.zeros(2, dtype=torch.int64, device="cuda:0")
+    lib = L.lib()
+
+    def launch():
+        L.check(lib.dwbc_track_episodes(L.ptr(rew), L.ptr(arm), L.ptr(dones), n, L.ptr(running), L.ptr(ring), L.ptr(pos), cap,
+                                        L.stream_ptr()), "dwbc_track_episodes")
+    for _ in range(50):
+        launch()
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+    ev[0].record()
+    for _ in range(launches):
+        launch()
+    ev[1].record()
+    graph = torch.cuda.CUDAGraph()                      # the same launches replayed from a graph, as in a captured rollout
+    with torch.cuda.graph(graph):
+        for _ in range(launches):
+            launch()
+    graph.replay()
+    ev[2].record()
+    graph.replay()
+    ev[3].record()
+    torch.cuda.synchronize()
+    return dict(eager=1e3 * ev[0].elapsed_time(ev[1]) / launches, graph=1e3 * ev[2].elapsed_time(ev[3]) / launches)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--hist", type=int, default=10, choices=[10, 20, 50], help="history_len (StateHistoryEncoder tsteps)")
     ap.add_argument("--envs", type=int, default=4096)
     ap.add_argument("--runs", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--track-episodes", type=int, default=0, help="C > 0: also run the arms with FusedPPO(track_episodes=C)")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     assert torch.cuda.is_available(), "graph_timing.py measures on a CUDA device"
@@ -69,13 +107,14 @@ def main():
     L._lib = counting                                   # FusedPPO / the env core / the storage bind L.lib() at construction
 
     arms = {}
-    for name in ("eager", "graphs"):
-        _, env, alg, pool = workload(args.hist, "tf32x3", args.envs)
-        env.set_obs_target(alg.storage.obs_row(0))
-        w = SimpleNamespace(env=env, alg=alg, pool=pool, obs=alg.storage.obs_row(0), last=None)
-        alg.cuda_graphs = name == "graphs"
-        rg = RolloutGraph(alg, env, physics=lambda t, w=w: w.env.bind_sim(**w.pool[t])) if name == "graphs" else None
-        arms[name] = dict(w=w, rg=rg, rows=[])
+    for track in ((0, args.track_episodes) if args.track_episodes else (0,)):
+        for mode in ("eager", "graphs"):
+            _, env, alg, pool = workload(args.hist, "tf32x3", args.envs, track_episodes=track)
+            env.set_obs_target(alg.storage.obs_row(0))
+            w = SimpleNamespace(env=env, alg=alg, pool=pool, obs=alg.storage.obs_row(0), last=None)
+            alg.cuda_graphs = mode == "graphs"
+            rg = RolloutGraph(alg, env, physics=lambda t, w=w: w.env.bind_sim(**w.pool[t])) if mode == "graphs" else None
+            arms[mode + ("+track" if track else "")] = dict(w=w, rg=rg, rows=[])
 
     def rollout(w):
         """bench.Workload.rollout: the loop RolloutGraph captures, obs_T of the previous iteration carried into storage row 0."""
@@ -120,19 +159,25 @@ def main():
         for arm in arms.values():
             iteration(arm, False)
     info0 = gpu_info()
-    for _ in range(args.runs):                          # alternating: eager, graphs, eager, ...
+    for _ in range(args.runs):                          # alternating: eager, graphs[, eager+track, graphs+track], eager, ...
         for arm in arms.values():
             iteration(arm, True)
+    tracker_us = {n: tracker_step_us(L, n, args.track_episodes) for n in (args.envs, 40000)} if args.track_episodes else None
     info1 = gpu_info()
     tma = tuple(bool(arm["w"].env._derived_state[:, 27].any()) for arm in arms.values())
     res = {"workload": f"bench.py flat: {args.envs} envs, history_len {args.hist}, T=40, tf32x3, 5 epochs x 4 mini-batches",
-           "k1_kernel": {(True, True): "TMA", (False, False): "warp-per-env"}.get(tma, f"differs between the arms: {tma}"),
+           "k1_kernel": "TMA" if all(tma) else "warp-per-env" if not any(tma) else f"differs between the arms: {tma}",
            "runs": args.runs, "warmup": args.warmup, "gpu_before": info0, "gpu_after": info1, "torch": torch.__version__}
     for name, arm in arms.items():
         rows = arm["rows"]
         res[name] = {k: dict(median=float(np.median([r[k] for r in rows])), min=float(min(r[k] for r in rows)),
                              max=float(max(r[k] for r in rows))) for k in rows[0]}
-    res["same_bits"] = bool(torch.equal(arms["eager"]["w"].alg.actor_critic.flat, arms["graphs"]["w"].alg.actor_critic.flat))
+    flat = [arm["w"].alg.actor_critic.flat for arm in arms.values()]
+    res["same_bits"] = all(torch.equal(flat[0], f) for f in flat[1:])
+    if args.track_episodes:
+        bufs = [arms[k]["w"].alg.episode_buffers() for k in ("eager+track", "graphs+track")]
+        res["track_episodes"] = dict(capacity=args.track_episodes, tracker_step_us=tracker_us, same_buffers=bufs[0] == bufs[1],
+                                     episodes_kept=len(bufs[0]["lenbuffer"]))
     line = json.dumps(res)
     print(line, flush=True)
     if args.out:

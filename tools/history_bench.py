@@ -55,9 +55,9 @@ def events_ms(fn, reps):
     return e0.elapsed_time(e1) / reps
 
 
-def workload(H, precision, n_envs=N_ENVS):
+def workload(H, precision, n_envs=N_ENVS, track_episodes=0):
     """bench.py's flat workload (same seeds, hyper-parameters and synthetic sim-state pool of T entries) at history_len H and n_envs envs:
-    (params, env core, FusedPPO with its storage, pool)."""
+    (params, env core, FusedPPO with its storage, pool).  track_episodes: FusedPPO's episode tracker (0: off, as in bench.py)."""
     import envstate as E
     from dwbc_b200 import synth
     from dwbc_b200.actor_critic import FlatActorCritic
@@ -71,7 +71,7 @@ def workload(H, precision, n_envs=N_ENVS):
     env = FusedWidowGo1Core(p, dev, state=st, seed=1000, sync_stats=False)
     env.update_command_curriculum()
     ac = FlatActorCritic(device=dev, seed=0, init_std=[[0.8, 1.0, 1.0] * 4 + [1.0] * 6], num_priv=24, num_hist=H, num_prop=76)
-    alg = FusedPPO(ac, device=dev, precision=precision, **HP)
+    alg = FusedPPO(ac, device=dev, precision=precision, track_episodes=track_episodes, **HP)
     alg.init_storage(n_envs, T, [p.num_obs], [None], [p.num_actions])
     alg.counter = 1500
     alg.generator = torch.Generator(device=dev)
