@@ -159,6 +159,7 @@ _SIGS = {
     "dwbc_ppo_minibatch_grad_sched": [vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp],
     "dwbc_clip_adam_step_table": [vp, vp, vp, vp, i64, i64, vp, i32, vp, vp, vp, vp],
     "dwbc_track_episodes": [vp, vp, vp, i32, vp, vp, vp, i32, vp],
+    "dwbc_policy_mean": [vp, vp, vp, i64, i32, vp, i32, i32, vp, vp],
 }
 EXPORTS = sorted(list(_SIGS) + ["dwbc_workspace_bytes", "dwbc_version", "dwbc_struct_sizes", "dwbc_launch_count", "dwbc_step_device_size"])
 

@@ -9,6 +9,7 @@ use the reference's key names and shapes, so checkpoints written by
 """
 from __future__ import annotations
 
+import ctypes as C
 import math
 from collections import OrderedDict
 from typing import List, Tuple
@@ -71,6 +72,39 @@ def manifest(num_prop=76, num_priv=24, num_hist=10, priv_dims=(64, 20), actor_di
     return m
 
 
+class PolicyMean:
+    """dwbc_policy_mean on a workspace of its own.  The tensor-core weight images stay in the workspace between calls and are rebuilt
+    when the key changes: rows, history flag, parameter buffer and its torch version (`load_state_dict` bumps it), network and precision,
+    and the observation layout that decides between the chains and the layer-wise path.  Parameters written by a kernel (the fused Adam
+    step) do not bump the version: a caller that cannot rule that out passes repack=True."""
+
+    def __init__(self):
+        self.ws, self.rows, self.key = None, 0, None
+
+    def reserve(self, ac, rows):
+        if self.ws is None or rows > self.rows or self.ws.device != ac.flat.device:
+            nbytes = L.lib().dwbc_workspace_bytes(C.addressof(ac.net_cfg), rows)
+            if nbytes < 0:
+                raise L.DwbcError("dwbc_workspace_bytes rejected the network configuration")
+            self.ws, self.rows, self.key = torch.zeros(nbytes // 4 + 64, device=ac.device), rows, None
+        return self.ws
+
+    def __call__(self, ac, obs, out, hist_encoding=False, repack=False):
+        """out [N, n_leg + n_arm] = the action mean of obs [N, >= num_obs] (float32, contiguous rows of stride obs.stride(0))."""
+        n, na = obs.shape[0], ac.num_leg_actions + ac.num_arm_actions
+        if obs.dim() != 2 or obs.shape[1] < ac.num_obs or obs.dtype != torch.float32:
+            raise L.DwbcError(f"observations must be float32 [N, >={ac.num_obs}], got {obs.dtype} {tuple(obs.shape)}")
+        if tuple(out.shape) != (n, na):
+            raise L.DwbcError(f"the mean output must be [{n}, {na}], got {tuple(out.shape)}")
+        ws = self.reserve(ac, n)
+        key = (n, bool(hist_encoding), ac.flat.data_ptr(), ac.flat._version, bytes(ac.net_cfg), obs.data_ptr() % 16, obs.stride(0) % 4)
+        packed = not repack and key == self.key
+        L.check(L.lib().dwbc_policy_mean(C.addressof(ac.net_cfg), L.ptr(ac.flat), L.ptr(obs, torch.float32), obs.stride(0), int(bool(hist_encoding)),
+                                         L.ptr(out, torch.float32), n, int(packed), L.ptr(ws), L.stream_ptr()), "dwbc_policy_mean")
+        self.key = key
+        return out
+
+
 class FlatActorCritic:
     is_recurrent = False
 
@@ -101,6 +135,7 @@ class FlatActorCritic:
         self.views = OrderedDict((n, self.flat[self.offsets[n]:self.offsets[n] + math.prod(s)].view(s)) for n, s in self.manifest)
         self.reset_parameters(init_std, seed)
         self.net_cfg = self._make_net_cfg()
+        self._mean = PolicyMean()
 
     # -- torch default init of nn.Linear / nn.Conv1d (kaiming_uniform(a=sqrt 5) == U(+-1/sqrt(fan_in))), AC relies on it
     def reset_parameters(self, init_std=None, seed=None):
@@ -184,6 +219,13 @@ class FlatActorCritic:
         for k, v in sd.items():
             if k in self.views:
                 self.views[k].copy_(torch.as_tensor(v).to(self.device).reshape(self.views[k].shape))
+
+    def act_inference(self, observations, hist_encoding=False):
+        """AC:347-349: the action mean [N, n_leg + n_arm] of observations [N, >= num_obs], by the actor alone (dwbc_policy_mean) at the
+        precision in net_cfg.  The weight images are rebuilt on every call: a training step may have moved the parameters in place."""
+        obs = observations.contiguous()
+        out = torch.empty(obs.shape[0], self.num_leg_actions + self.num_arm_actions, device=self.device)
+        return self._mean(self, obs, out, hist_encoding, repack=True)
 
     def parameters(self):
         return list(self.views.values())

@@ -850,7 +850,8 @@ struct C2Chains {
 // C2_PACK_FLOATS).  A network that passes chain_usable can still fail the latter (e.g. three 128-wide backbone layers per network: 38
 // images in the update); it then runs layer-wise like any network with a layer wider than 128.
 // what: 0 = dwbc_policy_act (`hist`: the latent comes from the history encoder, in p.zh), 1 = dwbc_critic_values, 2 =
-// dwbc_ppo_minibatch_grad (`idx`: its gather index).  `sms`: the SM count the rollout's split into one program per head follows.
+// dwbc_ppo_minibatch_grad (`idx`: its gather index), 3 = dwbc_policy_mean (the actor programs of 0 alone, `hist` as there).  `sms`: the SM
+// count the rollout's split into one program per head follows.
 static bool plan_chains(C2Chains& c, int what, const DwbcNetCfg& n, const float* P, const float* obs, const int64_t* idx, int64_t obs_stride,
                         bool hist, float* values, const Plan& p, int rows, int sms) {
   if (!chain_usable(n, p, obs, obs_stride)) return false;
@@ -865,6 +866,13 @@ static bool plan_chains(C2Chains& c, int what, const DwbcNetCfg& n, const float*
   } else if (what == 1) {
     const bool split = 2 * tiles <= sms;
     rc = build_forward(n, P, obs, nullptr, obs_stride, nullptr, 0, p, values, false, 0, nullptr, &B[0], nullptr, split ? &B[1] : nullptr);
+    c.nprog = split ? 2 : 1;
+  } else if (what == 3) {
+    // Every op of these programs is an op of mode 0's actor programs with the same operands; each program owns whole row tiles, and a
+    // trunk stored to p.ab and reloaded for the second head is the fp32 value the split program keeps in its tile.  So the means do not
+    // depend on where the two modes split (4 * tiles vs 2 * tiles <= sms).
+    const bool split = 2 * tiles <= sms;
+    rc = build_forward(n, P, obs, nullptr, obs_stride, hist ? p.zh : nullptr, zld, p, values, false, 1, &B[0], nullptr, split ? &B[1] : nullptr);
     c.nprog = split ? 2 : 1;
   } else {
     rc = build_forward(n, P, obs, idx, obs_stride, nullptr, zld, p, values, true, 2, &B[0], &B[1]);
@@ -958,6 +966,43 @@ extern "C" int dwbc_policy_act(const DwbcNetCfg* net, const float* params, const
   act_finalize_kernel<<<(rows + 127) / 128, 128, 0, st>>>(p.mean, p.mean_ld, params + n.off_std, eps, actions, log_prob, mean, sigma, rows,
                                                            n.n_leg, n.n_leg + n.n_arm);
   DWBC_LAUNCH_CHECK();
+  return DWBC_OK;
+}
+
+// The actor half of dwbc_policy_act: the same ops on the same operands, without the critic programs and the sampling epilogue.  It takes
+// the chains exactly when dwbc_policy_act would (mode 0 is planned first: a network whose rollout programs overflow the pack list runs
+// layer-wise there, so it must here too), which keeps `mean` bitwise equal to dwbc_policy_act's.
+extern "C" int dwbc_policy_mean(const DwbcNetCfg* net, const float* params, const float* obs, int64_t obs_stride, int32_t hist_encoding,
+                                float* mean, int32_t rows, int32_t weights_packed, void* workspace, dwbc_stream_t stream) {
+  TRY(check_net(net));
+  if (!params || !obs || !mean || !workspace || rows <= 0) return DWBC_ERR_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  const DwbcNetCfg& n = *net;
+  Plan p = make_plan(n, rows, workspace);
+  const int zld = (int)align_up(p.latent, 4), n_act = n.n_leg + n.n_arm;
+  const bool x3 = mlp_precision == 2;
+  const int sms = c2_sm_count();
+  bool chains;
+  {
+    C2Chains act(p.wpack, rows, x3);
+    chains = plan_chains(act, 0, n, params, obs, nullptr, obs_stride, hist_encoding != 0, p.value, p, rows, sms);
+  }
+  C2Chains ch(p.wpack, rows, x3);
+  if (chains && plan_chains(ch, 3, n, params, obs, nullptr, obs_stride, hist_encoding != 0, p.value, p, rows, sms)) {
+    if (hist_encoding) TRY(hist_latent_only(n, params, obs, nullptr, obs_stride, rows, p, p.zh, zld, st));
+    if (!weights_packed) TRY(launch_pack2(ch.pl, st));
+    const C2Prog* prs[2] = {&ch.b[0].pr, &ch.b[1].pr};
+    FinArgs f{};
+    f.mean_out = mean; f.n_leg = n.n_leg; f.n_act = n_act; f.rows = rows;
+    return launch_chain2n(prs, ch.nprog, f, x3, p.queue, st);
+  }
+  if (chains) return DWBC_ERR_UNSUPPORTED;          // (cannot happen: the actor programs are a subset of mode 0's; see plan_chains)
+  if (hist_encoding) TRY(hist_forward(n, params, obs, nullptr, obs_stride, rows, p, st));
+  else TRY(priv_forward(n, params, obs, nullptr, obs_stride, rows, p, st));
+  TRY(actor_forward(n, params, obs, nullptr, obs_stride, rows, hist_encoding ? p.zh : p.priv[n.n_priv_layers - 1], zld, p, st));
+  if (cudaMemcpy2DAsync(mean, sizeof(float) * n_act, p.mean, sizeof(float) * p.mean_ld, sizeof(float) * n_act, rows, cudaMemcpyDeviceToDevice, st) !=
+      cudaSuccess)
+    return DWBC_ERR_LAUNCH;
   return DWBC_OK;
 }
 
@@ -1210,20 +1255,21 @@ extern "C" int dwbc_debug_gemm(int mode, int tc, const float* A, int64_t lda, co
 
 // The chain PROGRAMS a call would launch, described without launching anything (host code only, no GPU; every pointer is formed from the
 // fake bases below and never dereferenced).  what: 0 = dwbc_policy_act, 1 = dwbc_critic_values, 2 = forward + loss of dwbc_ppo_minibatch_grad,
-// 3 = its backward launch.  out = [nprog, pack items, then per program: n_ops, n_loads, then per op: N, kpad, act, fin, fin_c, out_col0,
-// has_global_output, output_is_tile_image].  Returns the number of ints written, or a negative error code (DWBC_ERR_UNSUPPORTED: the
+// 3 = its backward launch, 4 = dwbc_policy_mean (when dwbc_policy_act runs on the chains).  out = [nprog, pack items, then per program:
+// n_ops, n_loads, then per op: N, kpad, act, fin, fin_c, out_col0, has_global_output, output_is_tile_image].  Returns the number of ints written, or a negative error code (DWBC_ERR_UNSUPPORTED: the
 // configuration does not run on the fused chains).  tests/test_host_cpu.py pins the program structure with it.
 extern "C" int dwbc_debug_describe_chain(const DwbcNetCfg* net, int32_t rows, int what, int hist_encoding, int sms, int32_t* out, int32_t out_len) {
   TRY(check_net(net));
-  if (rows <= 0 || what < 0 || what > 3 || sms <= 0 || !out) return DWBC_ERR_ARG;
+  if (rows <= 0 || what < 0 || what > 4 || sms <= 0 || !out) return DWBC_ERR_ARG;
   const DwbcNetCfg& n = *net;
   float* const ws = reinterpret_cast<float*>(uintptr_t(1) << 40);
   const float* const P = reinterpret_cast<const float*>(uintptr_t(2) << 40);
   const float* const obs = reinterpret_cast<const float*>(uintptr_t(3) << 40);
-  const int64_t* const idx = what >= 2 ? reinterpret_cast<const int64_t*>(uintptr_t(4) << 40) : nullptr;
+  const int64_t* const idx = what == 2 || what == 3 ? reinterpret_cast<const int64_t*>(uintptr_t(4) << 40) : nullptr;
   Plan p = make_plan(n, rows, ws);
   C2Chains ch(p.wpack, rows, mlp_precision == 2);
-  if (!plan_chains(ch, what < 2 ? what : 2, n, P, obs, idx, n.num_obs, hist_encoding != 0, p.value, p, rows, sms)) return DWBC_ERR_UNSUPPORTED;
+  const int mode = what < 2 ? what : (what == 4 ? 3 : 2);
+  if (!plan_chains(ch, mode, n, P, obs, idx, n.num_obs, hist_encoding != 0, p.value, p, rows, sms)) return DWBC_ERR_UNSUPPORTED;
   const C2Builder* prs = what == 3 ? ch.b + 2 : ch.b;
   int k = 0;
   auto put = [&](int v) { if (k < out_len) out[k] = v; ++k; };

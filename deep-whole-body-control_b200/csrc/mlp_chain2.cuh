@@ -82,7 +82,7 @@ static_assert(sizeof(C2Prog) % 16 == 0, "copied to shared memory in 16-byte piec
 // everything the epilogue hooks need (AC:326-345, PPO:166-221)
 struct FinArgs {
   const float* std;                                          // [n_act]
-  // FIN_ACT (rollout): a = mu + std * eps
+  // FIN_ACT (rollout): a = mu + std * eps.  actions == nullptr: the mean only (dwbc_policy_mean; eps, log_prob, sigma_out unread)
   const float* eps; float* actions; float* log_prob; float* mean_out; float* sigma_out;
   // FIN_PPO / FIN_VALUE / FIN_REG (update)
   const int64_t* idx;                                        // mini-batch gather index (storage row of mini-batch row r)
@@ -294,6 +294,7 @@ __device__ __forceinline__ void c2_fin_act(const FinArgs& f, int c, int64_t m, b
   if (!on) return;
   const int off = c == 0 ? 0 : f.n_leg, cnt = c == 0 ? f.n_leg : f.n_act - f.n_leg;
   const bool vec2 = ((f.n_act | f.n_leg) & 1) == 0;
+  if (f.actions == nullptr) { c2_st_group(f.mean_out + m * f.n_act + off, cnt, vec2, v); return; }
   float sg[C2_GRP], ep[C2_GRP], ac[C2_GRP], mu[C2_GRP];
   c2_ld_group(f.std + off, cnt, vec2, sg);
   c2_ld_group(f.eps + m * f.n_act + off, cnt, vec2, ep);

@@ -90,16 +90,9 @@ class FusedActorCritic(nn.Module):
         return lib
 
     def act_inference(self, observations, hist_encoding=False):
-        """AC:347-349: the action mean (eps = 0, so actions == mean)."""
-        obs = observations.contiguous()
-        n = obs.shape[0]
-        lib = self._scratch(n)
-        eps, act, mu, sg, val, lp = self._tmp
-        eps.zero_()
-        L.check(lib.dwbc_policy_act(C.addressof(self.core.net_cfg), L.ptr(self.core.flat), L.ptr(obs, torch.float32), obs.stride(0), L.ptr(eps),
-                                    int(bool(hist_encoding)), L.ptr(act), L.ptr(val), L.ptr(lp), L.ptr(mu), L.ptr(sg), n, 0, L.ptr(self._ws),
-                                    L.stream_ptr()), "dwbc_policy_act")
-        return mu.clone()
+        """AC:347-349: the action mean, by the actor alone (FlatActorCritic.act_inference: dwbc_policy_mean, the bits of dwbc_policy_act's
+        mean)."""
+        return self.core.act_inference(observations, hist_encoding)
 
     def evaluate(self, critic_observations, **kwargs):
         """AC:351-353."""

@@ -360,6 +360,14 @@ int dwbc_policy_act(const DwbcNetCfg* net, const float* params, const float* obs
                     int32_t hist_encoding, float* actions, float* values, float* log_prob, float* mean, float* sigma,
                     int32_t rows, int32_t weights_packed, void* workspace, dwbc_stream_t stream);
 
+/* The actor forward alone (AC:204-217; act_inference AC:347-349): obs[rows, obs_stride] -> mean[rows, n_leg + n_arm], the tanh outputs of
+ * the leg and arm heads, on the privileged-encoder latent or, with hist_encoding, the history-encoder latent.  No noise is read and no
+ * critic, sigma or log-prob is computed.  On the same network, precision, parameters, observations, hist_encoding and rows, `mean` is
+ * bitwise equal to the mean output of dwbc_policy_act.  weights_packed as there, but the images differ: 1 only after a dwbc_policy_mean
+ * call (never after dwbc_policy_act) on the same workspace, net, rows and parameters.  The workspace is dwbc_workspace_bytes(net, rows). */
+int dwbc_policy_mean(const DwbcNetCfg* net, const float* params, const float* obs, int64_t obs_stride, int32_t hist_encoding,
+                     float* mean, int32_t rows, int32_t weights_packed, void* workspace, dwbc_stream_t stream);
+
 /* critic only (PPO:148-150 last_values; AC:351-353) */
 int dwbc_critic_values(const DwbcNetCfg* net, const float* params, const float* obs, int64_t obs_stride, float* values,
                        int32_t rows, void* workspace, dwbc_stream_t stream);
