@@ -17,6 +17,9 @@ MAX_DOF, MAX_TERMS, MAX_IDX, MAX_SLOTS, NUM_METRICS, RAND_COLS, MAX_LAYERS = 24,
 GS, DS = 28, 72
 # device scratch sizes (dwbc.h): dwbc_clip_adam_step norm partials, dwbc_gae stats (doubles)
 NORM_SCRATCH, GAE_STATS = 592, 4 + 2 * 1024
+# dwbc_ppo_minibatch_grad_diag's diag_out[DIAG_N] slots, and dwbc_explained_variance's scratch (doubles)
+DIAG_KL_LEG, DIAG_KL_ARM, DIAG_CLIP_LEG, DIAG_CLIP_ARM, DIAG_GRAD_NORM, DIAG_N = 0, 1, 2, 3, 4, 5
+EV_SCRATCH = 2 + 8 * 256
 GS_COL = dict(commands=0, goal_timer=3, traj_timesteps=4, traj_total_timesteps=5, ee_start_sphere=6, ee_goal_sphere=9,
               ee_goal_cart=12, curr_ee_goal_sphere=15, curr_ee_goal_cart=18, ee_goal_delta_orn_euler=21, ee_goal_orn_euler=24)
 DS_COL = dict(base_lin_vel=0, base_ang_vel=3, base_yaw_euler=6, base_yaw_quat=9, last_root_vel=13, feet_air_time=19,
@@ -160,6 +163,8 @@ _SIGS = {
     "dwbc_clip_adam_step_table": [vp, vp, vp, vp, i64, i64, vp, i32, vp, vp, vp, vp],
     "dwbc_track_episodes": [vp, vp, vp, i32, vp, vp, vp, i32, vp],
     "dwbc_policy_mean": [vp, vp, vp, i64, i32, vp, i32, i32, vp, vp],
+    "dwbc_ppo_minibatch_grad_diag": [vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp],
+    "dwbc_explained_variance": [vp, vp, i64, vp, vp, vp],
 }
 EXPORTS = sorted(list(_SIGS) + ["dwbc_workspace_bytes", "dwbc_version", "dwbc_struct_sizes", "dwbc_launch_count", "dwbc_step_device_size"])
 

@@ -119,9 +119,58 @@ __global__ void store_rewards_kernel(const float* __restrict__ rew, const float*
   if (dones) dones[i] = resets[i] ? 1 : 0;
 }
 
+// Explained variance: per channel c the block's sums of R, R^2, R - V and (R - V)^2 (each shifted by row 0's value) in double -> slot 8 b + 4 c + k of scratch (after the
+// counter); the last block adds the slots up in block order.
+constexpr int EV_BLOCK = 256;
+__global__ void __launch_bounds__(EV_BLOCK)
+explained_variance_kernel(const float* __restrict__ values, const float* __restrict__ returns, int64_t rows, double* scratch, float* out) {
+  __shared__ double red[8][EV_BLOCK / 32];
+  // shifted by row 0's R and R - V: no cancellation against a large mean, and exactly 0 for a constant channel
+  const double k[4] = {returns[0], returns[0] - (double)values[0], returns[1], returns[1] - (double)values[1]};
+  double v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  for (int64_t j = (int64_t)blockIdx.x * EV_BLOCK + threadIdx.x; j < rows; j += (int64_t)gridDim.x * EV_BLOCK) {
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+      const double R = __ldg(returns + 2 * j + c), r = R - k[2 * c], e = (R - (double)__ldg(values + 2 * j + c)) - k[2 * c + 1];
+      v[4 * c] += r; v[4 * c + 1] += r * r; v[4 * c + 2] += e; v[4 * c + 3] += e * e;
+    }
+  }
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const double s = warp_sum(v[k]);
+    if (lane == 0) red[k][w] = s;
+  }
+  __syncthreads();
+  double* part = scratch + 2;
+  if (threadIdx.x < 8) {
+    double s = 0.0;
+    for (int i = 0; i < EV_BLOCK / 32; ++i) s += red[threadIdx.x][i];
+    part[8 * blockIdx.x + threadIdx.x] = s;
+  }
+  if (!last_block(reinterpret_cast<unsigned*>(scratch)) || threadIdx.x >= 2) return;
+  const int c = threadIdx.x;
+  double t[4] = {0, 0, 0, 0};
+  for (int b = 0; b < (int)gridDim.x; ++b)
+    for (int k = 0; k < 4; ++k) t[k] += __ldcg(part + 8 * b + 4 * c + k);
+  const double n = (double)rows;
+  const double var_r = fmax(t[1] / n - (t[0] / n) * (t[0] / n), 0.0), var_e = fmax(t[3] / n - (t[2] / n) * (t[2] / n), 0.0);
+  out[c] = var_r > 0.0 ? (float)(1.0 - var_e / var_r) : __int_as_float(0x7fc00000);
+}
+
 }  // namespace dwbc
 
 using namespace dwbc;
+
+extern "C" int dwbc_explained_variance(const float* values, const float* returns, int64_t rows, double* scratch, float* out,
+                                       dwbc_stream_t stream) {
+  if (!values || !returns || !scratch || !out || rows <= 0) return DWBC_ERR_ARG;
+  const int64_t blocks = (rows + EV_BLOCK - 1) / EV_BLOCK;
+  const int grid = blocks < DWBC_EV_MAX_BLOCKS ? (int)blocks : DWBC_EV_MAX_BLOCKS;   // grid-stride loops cover the rest
+  explained_variance_kernel<<<grid, EV_BLOCK, 0, (cudaStream_t)stream>>>(values, returns, rows, scratch, out);
+  DWBC_LAUNCH_CHECK();
+  return DWBC_OK;
+}
 
 extern "C" int dwbc_gae(const float* rewards, const float* values, const uint8_t* dones, const float* last_values,
                         float* returns, float* advantages, double* stats, int32_t T, int32_t N, float gamma, float lam,

@@ -60,7 +60,7 @@ struct Plan {
   float* hw[3]; float* hwl;                // re-packed weights: conv i [c_i][k_i*ld[i]], linear_output [32][36]
   float* wpack;                            // packed weight images of the fused chain kernels (mlp_chain2.cuh)
   int* queue;                              // counters, zero between launches: [0..1] work queue of the chain kernel, [2] ppo_loss_kernel, [3]
-                                           // dagger_loss_kernel
+                                           // dagger_loss_kernel, [4] ppo_diag_kernel
   float* loss_part;                        // per-block / per-(tile, warp) partial sums of the loss kernels
   float* wpart;                            // per-(GEMM, slab) / per-(split) partials of the weight gradients (wpart_floats)
   // gradients
@@ -449,12 +449,15 @@ static void chain_head(C2Builder& b, const float* P, const float* trunk, int tru
 
 // Programs of the forward pass.  z_hist == nullptr: latent from the privileged encoder (computed inside the chain); else the history
 // latent [rows, zld].  `loss`: update mode (hooks FIN_REG / FIN_PPO / FIN_VALUE), else rollout mode (FIN_ACT), else none (fin_mode 0).
+// keep_mean: the heads' last ops also write the means to Plan::mean in update mode (through the ops' ordinary global output), at row
+// stride n_act: the vector stores of an op need 16-byte aligned rows, which stride n_act gives whenever they are taken (n_act and the
+// head's N multiples of 4 make n_leg one too), so any action split the update runs on the chains still does.
 // With A2 / C2 (inference only: `store` off) the two heads of a network become TWO programs that each recompute the short common part
 // (encoder + backbone): a 4096-row rollout then is 4 programs x 32 tiles = 128 one-tile items of at most 6 ops on 128 SMs instead of
 // 2 x 32 items of 9 / 7 ops on 64 SMs -- the launch is as long as its longest item.
 static int build_forward(const DwbcNetCfg& n, const float* P, const float* obs, const int64_t* idx, int64_t obs_stride, const float* z_hist, int zld,
                          const Plan& p, float* value, bool store, int fin_mode, C2Builder* A, C2Builder* C, C2Builder* A2 = nullptr,
-                         C2Builder* C2 = nullptr) {
+                         C2Builder* C2 = nullptr, bool keep_mean = false) {
   const int Lld = (int)align_up(p.latent, 4);
   if ((A2 || C2) && store) return DWBC_ERR_ARG;
   if (A) {
@@ -489,13 +492,14 @@ static int build_forward(const DwbcNetCfg& n, const float* P, const float* obs, 
       return in;
     };
     const int fin = fin_mode == 2 ? FIN_PPO : (fin_mode == 1 ? FIN_ACT : FIN_NONE);
-    float* mean = fin_mode == 0 ? p.mean : nullptr;
+    float* mean = fin_mode == 0 || keep_mean ? p.mean : nullptr;      // keep_mean: the update's means for ppo_diag_kernel
+    const int64_t mean_ld = fin_mode == 0 ? p.mean_ld : n.n_leg + n.n_arm;
     const int in = common(*A, A2 == nullptr);
-    chain_head(*A, P, p.ab[na - 1], in, false, in, n.n_leg_layers, n.leg_dims, n.n_leg, n.off_aleg_w, n.off_aleg_b, p.al, store, mean, p.mean_ld, ACT_TANH, fin, 0);
+    chain_head(*A, P, p.ab[na - 1], in, false, in, n.n_leg_layers, n.leg_dims, n.n_leg, n.off_aleg_w, n.off_aleg_b, p.al, store, mean, mean_ld, ACT_TANH, fin, 0);
     C2Builder& Barm = A2 ? *A2 : *A;
     if (A2) common(*A2, false);
     chain_head(Barm, P, p.ab[na - 1], in, A2 == nullptr, in, n.n_arm_layers, n.arm_dims, n.n_arm, n.off_aarm_w, n.off_aarm_b, p.aa, store,
-               mean ? mean + n.n_leg : nullptr, p.mean_ld, ACT_TANH, fin, 1);
+               mean ? mean + n.n_leg : nullptr, mean_ld, ACT_TANH, fin, 1);
     A->finish();
     if (A2) A2->finish();
     if (!A->ok || (A2 && !A2->ok)) return DWBC_ERR_UNSUPPORTED;
@@ -586,9 +590,9 @@ __global__ void __launch_bounds__(128) ppo_loss_kernel(const LossArgs a) {
     const float* act = a.actions + src * a.n_act;
     float lp[2] = {0.0f, 0.0f}, ent[2] = {0.0f, 0.0f};
     for (int i = 0; i < a.n_act; ++i) {
-      const float sg = a.std[i], d = act[i] - mu[i];
+      const float sg = a.std[i];
       const int c = i < a.n_leg ? 0 : 1;
-      lp[c] += -(d * d) / (2.0f * (sg * sg)) - logf(sg) - LOG_SQRT_2PI;          // AC:341-345
+      lp[c] += ppo_logp_term(act[i], mu[i], sg, logf(sg));                        // AC:341-345
       ent[c] += 0.5f + LOG_SQRT_2PI + logf(sg);                                  // AC:326-331 (0.5 log 2pi == log sqrt 2pi)
     }
     const float a0 = a.adv[2 * src], a1 = a.adv[2 * src + 1];
@@ -723,6 +727,63 @@ __global__ void __launch_bounds__(128) dagger_loss_kernel(const float* __restric
   *loss += t;
 }
 
+// ---- PPO update diagnostics (dwbc_ppo_minibatch_grad_diag) ----------------------------------------
+// Per channel c (leg = actions [0, n_leg), arm = the rest), over the M rows of a mini-batch:
+//   approx_kl[c]     = mean_rows sum_i log(sg_new / sg_old + 1e-5) + (sg_old^2 + (mu_old - mu_new)^2) / (2 sg_new^2) - 0.5  (rsl_rl's KL)
+//   clip_fraction[c] = share of rows whose ratio lies outside [1 - clip, 1 + clip]
+// The ratio is the loss's: ppo_logp_term summed in index order over the same new means, std and stored rows.  The KL terms are evaluated
+// and summed in double.  One partial per 128-row block, added up in block order by the last block.
+static_assert(DWBC_DIAG_KL_ARM == DWBC_DIAG_KL_LEG + 1 && DWBC_DIAG_CLIP_LEG == DWBC_DIAG_KL_LEG + 2 && DWBC_DIAG_CLIP_ARM == DWBC_DIAG_KL_LEG + 3,
+              "ppo_diag_kernel writes its four means to consecutive slots");
+struct DiagArgs {
+  const float* mean; int mean_ld;         // new means [rows, mean_ld] (the forward's)
+  const float* std;                       // new sigma: the std parameters the forward used
+  const float* actions; const float* old_logp; const float* old_mu; const float* old_sigma; const int64_t* idx;
+  float* out;                             // [DWBC_DIAG_KL_LEG .. DWBC_DIAG_CLIP_ARM] are written
+  double* part; unsigned* ticket;         // [blocks][4] partials
+  int rows, n_leg, n_act;
+  float clip;
+};
+
+__global__ void __launch_bounds__(128) ppo_diag_kernel(const DiagArgs a) {
+  __shared__ double red[4][4];
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  double v[4] = {0.0, 0.0, 0.0, 0.0};                                            // kl leg, kl arm, outside leg, outside arm
+  if (r < a.rows) {
+    const int64_t src = a.idx ? a.idx[r] : r;
+    const float* mu = a.mean + (int64_t)r * a.mean_ld;
+    const float* act = a.actions + src * a.n_act;
+    const float* omu = a.old_mu + src * a.n_act;
+    const float* osg = a.old_sigma + src * a.n_act;
+    float lp[2] = {0.0f, 0.0f};
+    for (int i = 0; i < a.n_act; ++i) {
+      const float sg = a.std[i];
+      const int c = i < a.n_leg ? 0 : 1;
+      lp[c] += ppo_logp_term(act[i], mu[i], sg, logf(sg));
+      const double sn = sg, so = osg[i], dm = (double)omu[i] - (double)mu[i];
+      v[c] += log(sn / so + 1e-5) + (so * so + dm * dm) / (2.0 * sn * sn) - 0.5;
+    }
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+      const float ratio = expf(lp[c] - a.old_logp[2 * src + c]);
+      v[2 + c] = (ratio >= 1.0f - a.clip && ratio <= 1.0f + a.clip) ? 0.0 : 1.0;
+    }
+  }
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const double s = warp_sum(v[k]);
+    if (lane == 0) red[k][w] = s;
+  }
+  __syncthreads();
+  const int q = threadIdx.x;
+  if (q < 4) a.part[(int64_t)blockIdx.x * 4 + q] = (red[q][0] + red[q][1]) + (red[q][2] + red[q][3]);
+  if (!last_block(a.ticket) || q >= 4) return;
+  double s = 0.0;
+  for (int b = 0; b < (int)gridDim.x; ++b) s += __ldcg(a.part + (int64_t)b * 4 + q);
+  a.out[DWBC_DIAG_KL_LEG + q] = (float)(s / (double)a.rows);
+}
+
 // ---- backward -----------------------------------------------------------------------------------
 // Backward of one head: Linear(+ELU) x nl, then Linear -> out.  G_out = d/d(pre-activation of the
 // last layer) [rows, n_out].  Accumulates weight grads into `grad`, and adds the head's
@@ -853,7 +914,7 @@ struct C2Chains {
 // dwbc_ppo_minibatch_grad (`idx`: its gather index), 3 = dwbc_policy_mean (the actor programs of 0 alone, `hist` as there).  `sms`: the SM
 // count the rollout's split into one program per head follows.
 static bool plan_chains(C2Chains& c, int what, const DwbcNetCfg& n, const float* P, const float* obs, const int64_t* idx, int64_t obs_stride,
-                        bool hist, float* values, const Plan& p, int rows, int sms) {
+                        bool hist, float* values, const Plan& p, int rows, int sms, bool keep_mean = false) {
   if (!chain_usable(n, p, obs, obs_stride)) return false;
   const int tiles = (rows + TC_M - 1) / TC_M, zld = (int)align_up(p.latent, 4);
   C2Builder* B = c.b;
@@ -875,7 +936,7 @@ static bool plan_chains(C2Chains& c, int what, const DwbcNetCfg& n, const float*
     rc = build_forward(n, P, obs, nullptr, obs_stride, hist ? p.zh : nullptr, zld, p, values, false, 1, &B[0], nullptr, split ? &B[1] : nullptr);
     c.nprog = split ? 2 : 1;
   } else {
-    rc = build_forward(n, P, obs, idx, obs_stride, nullptr, zld, p, values, true, 2, &B[0], &B[1]);
+    rc = build_forward(n, P, obs, idx, obs_stride, nullptr, zld, p, values, true, 2, &B[0], &B[1], nullptr, nullptr, keep_mean);
     if (rc == DWBC_OK) rc = build_backward(n, P, p, B[2], B[3]);
     c.nprog = 2;
   }
@@ -1031,11 +1092,14 @@ extern "C" int dwbc_hist_latent(const DwbcNetCfg* net, const float* params, cons
   return hist_latent_only(*net, params, obs, nullptr, obs_stride, rows, p, out, ld_out, (cudaStream_t)stream);
 }
 
-// sched: optional device (priv_reg_coef, mixing_ratio, torque_supervision_weight) read by the loss kernels in place of hp's fields
+// sched: optional device (priv_reg_coef, mixing_ratio, torque_supervision_weight) read by the loss kernels in place of hp's fields.
+// diag_out: optional (dwbc_ppo_minibatch_grad_diag): the forward also keeps the new means, and ppo_diag_kernel runs behind the loss.
 static int ppo_minibatch_grad(const DwbcNetCfg* net, const float* params, const DwbcStorage* s, const int64_t* idx, int32_t M,
-                              const DwbcPpoHyper* hp, const float* sched, float* grad, float* losses_out, void* workspace, dwbc_stream_t stream) {
+                              const DwbcPpoHyper* hp, const float* sched, const float* old_mu, const float* old_sigma, float* grad,
+                              float* losses_out, float* diag_out, void* workspace, dwbc_stream_t stream) {
   TRY(check_net(net));
   if (!params || !s || !idx || !hp || !grad || !losses_out || !workspace || M <= 0) return DWBC_ERR_ARG;
+  if (diag_out && (!old_mu || !old_sigma)) return DWBC_ERR_ARG;
   if (!s->observations || !s->actions || !s->values || !s->returns || !s->advantages || !s->log_prob) return DWBC_ERR_ARG;
   // torque supervision is on when the storage carries its three tensors (RS:82-84); then the arm coefficients are needed too
   if (s->target_arm_torques && (!s->current_arm_dof_pos || !s->current_arm_dof_vel || !hp->arm_coefs)) return DWBC_ERR_ARG;
@@ -1050,8 +1114,26 @@ static int ppo_minibatch_grad(const DwbcNetCfg* net, const float* params, const 
   // of all four programs are packed by ONE launch (the parameters are constant within a mini-batch).
   const bool x3 = mlp_precision == 2;
   C2Chains ch(p.wpack, rows, x3);
-  const bool chains = plan_chains(ch, 2, n, P, s->observations, idx, s->obs_stride, false, p.value, p, rows, 0);
+  const bool chains = plan_chains(ch, 2, n, P, s->observations, idx, s->obs_stride, false, p.value, p, rows, 0, diag_out != nullptr);
+  if (diag_out && !chains) {
+    // the diagnostics must never move an update off the chains (other rounding, other speed): refuse rather than fall back
+    C2Chains plain(p.wpack, rows, x3);
+    if (plan_chains(plain, 2, n, P, s->observations, idx, s->obs_stride, false, p.value, p, rows, 0)) return DWBC_ERR_UNSUPPORTED;
+  }
   if (cudaMemsetAsync(grad, 0, sizeof(float) * n.num_params, st) != cudaSuccess) return DWBC_ERR_LAUNCH;
+  // the diagnostics of this mini-batch over the forward's means, which both paths leave in Plan::mean (the chains only when asked to: the
+  // heads' last ops then write their outputs there at row stride n_act, the layer-wise forward at mean_ld)
+  auto diag = [&](int mean_ld) -> int {
+    if (!diag_out) return DWBC_OK;
+    DiagArgs d{};
+    d.mean = p.mean; d.mean_ld = mean_ld; d.std = P + n.off_std;
+    d.actions = s->actions; d.old_logp = s->log_prob; d.old_mu = old_mu; d.old_sigma = old_sigma; d.idx = idx;
+    d.out = diag_out; d.part = reinterpret_cast<double*>(p.loss_part); d.ticket = reinterpret_cast<unsigned*>(p.queue + 4);
+    d.rows = rows; d.n_leg = n.n_leg; d.n_act = n.n_leg + n.n_arm; d.clip = hp->clip_param;
+    ppo_diag_kernel<<<(rows + 127) / 128, 128, 0, st>>>(d);
+    DWBC_LAUNCH_CHECK();
+    return DWBC_OK;
+  };
 
   // forward (the reference evaluates the actor 3x and the priv encoder 3x per mini-batch,
   // PPO:166,174,230; identical values, so each is evaluated once here)
@@ -1071,6 +1153,7 @@ static int ppo_minibatch_grad(const DwbcNetCfg* net, const float* params, const 
     f.ts_w = hp->torque_supervision_weight; f.sched = sched;
     TRY(launch_pack2(ch.pl, st));
     TRY(launch_chain2(&ch.b[0].pr, &ch.b[1].pr, f, x3, p.queue, st));
+    TRY(diag(n.n_leg + n.n_arm));
     TRY(launch_chain2(&ch.b[2].pr, &ch.b[3].pr, FinArgs{}, x3, p.queue, st, true));      // downwards: the last tiles are still in L2
     return weight_gradients(n, grad, s, idx, rows, p, st);
   }
@@ -1090,6 +1173,7 @@ static int ppo_minibatch_grad(const DwbcNetCfg* net, const float* params, const 
   a.ts_w = hp->torque_supervision_weight; a.sched = sched;
   ppo_loss_kernel<<<(rows + 127) / 128, 128, 0, st>>>(a);
   DWBC_LAUNCH_CHECK();
+  TRY(diag(p.mean_ld));
 
   // ---- critic backward ----
   {
@@ -1159,14 +1243,21 @@ static int ppo_minibatch_grad(const DwbcNetCfg* net, const float* params, const 
 
 extern "C" int dwbc_ppo_minibatch_grad(const DwbcNetCfg* net, const float* params, const DwbcStorage* s, const int64_t* idx, int32_t M,
                                        const DwbcPpoHyper* hp, float* grad, float* losses_out, void* workspace, dwbc_stream_t stream) {
-  return ppo_minibatch_grad(net, params, s, idx, M, hp, nullptr, grad, losses_out, workspace, stream);
+  return ppo_minibatch_grad(net, params, s, idx, M, hp, nullptr, nullptr, nullptr, grad, losses_out, nullptr, workspace, stream);
 }
 
 extern "C" int dwbc_ppo_minibatch_grad_sched(const DwbcNetCfg* net, const float* params, const DwbcStorage* s, const int64_t* idx, int32_t M,
                                              const DwbcPpoHyper* hp, const float* sched, float* grad, float* losses_out, void* workspace,
                                              dwbc_stream_t stream) {
   if (!sched) return DWBC_ERR_ARG;
-  return ppo_minibatch_grad(net, params, s, idx, M, hp, sched, grad, losses_out, workspace, stream);
+  return ppo_minibatch_grad(net, params, s, idx, M, hp, sched, nullptr, nullptr, grad, losses_out, nullptr, workspace, stream);
+}
+
+extern "C" int dwbc_ppo_minibatch_grad_diag(const DwbcNetCfg* net, const float* params, const DwbcStorage* s, const int64_t* idx, int32_t M,
+                                            const DwbcPpoHyper* hp, const float* sched, const float* old_mu, const float* old_sigma, float* grad,
+                                            float* losses_out, float* diag_out, void* workspace, dwbc_stream_t stream) {
+  if (!old_mu || !old_sigma || !diag_out) return DWBC_ERR_ARG;
+  return ppo_minibatch_grad(net, params, s, idx, M, hp, sched, old_mu, old_sigma, grad, losses_out, diag_out, workspace, stream);
 }
 
 extern "C" int dwbc_dagger_minibatch_grad(const DwbcNetCfg* net, const float* params, const DwbcStorage* s, const int64_t* idx, int32_t M,
@@ -1255,21 +1346,22 @@ extern "C" int dwbc_debug_gemm(int mode, int tc, const float* A, int64_t lda, co
 
 // The chain PROGRAMS a call would launch, described without launching anything (host code only, no GPU; every pointer is formed from the
 // fake bases below and never dereferenced).  what: 0 = dwbc_policy_act, 1 = dwbc_critic_values, 2 = forward + loss of dwbc_ppo_minibatch_grad,
-// 3 = its backward launch, 4 = dwbc_policy_mean (when dwbc_policy_act runs on the chains).  out = [nprog, pack items, then per program:
+// 3 = its backward launch, 4 = dwbc_policy_mean (when dwbc_policy_act runs on the chains), 5 = forward + loss of dwbc_ppo_minibatch_grad_diag
+// (2 with the heads' means kept for the diagnostics).  out = [nprog, pack items, then per program:
 // n_ops, n_loads, then per op: N, kpad, act, fin, fin_c, out_col0, has_global_output, output_is_tile_image].  Returns the number of ints written, or a negative error code (DWBC_ERR_UNSUPPORTED: the
 // configuration does not run on the fused chains).  tests/test_host_cpu.py pins the program structure with it.
 extern "C" int dwbc_debug_describe_chain(const DwbcNetCfg* net, int32_t rows, int what, int hist_encoding, int sms, int32_t* out, int32_t out_len) {
   TRY(check_net(net));
-  if (rows <= 0 || what < 0 || what > 4 || sms <= 0 || !out) return DWBC_ERR_ARG;
+  if (rows <= 0 || what < 0 || what > 5 || sms <= 0 || !out) return DWBC_ERR_ARG;
   const DwbcNetCfg& n = *net;
   float* const ws = reinterpret_cast<float*>(uintptr_t(1) << 40);
   const float* const P = reinterpret_cast<const float*>(uintptr_t(2) << 40);
   const float* const obs = reinterpret_cast<const float*>(uintptr_t(3) << 40);
-  const int64_t* const idx = what == 2 || what == 3 ? reinterpret_cast<const int64_t*>(uintptr_t(4) << 40) : nullptr;
+  const int64_t* const idx = what == 2 || what == 3 || what == 5 ? reinterpret_cast<const int64_t*>(uintptr_t(4) << 40) : nullptr;
   Plan p = make_plan(n, rows, ws);
   C2Chains ch(p.wpack, rows, mlp_precision == 2);
   const int mode = what < 2 ? what : (what == 4 ? 3 : 2);
-  if (!plan_chains(ch, mode, n, P, obs, idx, n.num_obs, hist_encoding != 0, p.value, p, rows, sms)) return DWBC_ERR_UNSUPPORTED;
+  if (!plan_chains(ch, mode, n, P, obs, idx, n.num_obs, hist_encoding != 0, p.value, p, rows, sms, what == 5)) return DWBC_ERR_UNSUPPORTED;
   const C2Builder* prs = what == 3 ? ch.b + 2 : ch.b;
   int k = 0;
   auto put = [&](int v) { if (k < out_len) out[k] = v; ++k; };

@@ -200,6 +200,12 @@ template <int kRegs> __device__ __forceinline__ void c2_reg_inc() { asm volatile
 template <int kRegs> __device__ __forceinline__ void c2_reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs)); }
 __device__ __forceinline__ void c2_wbar() { __syncwarp(); asm volatile("bar.sync 1, %0;" ::"n"(C2_NW) : "memory"); }     // the worker warps
 constexpr float C2_LOG_SQRT_2PI = 0.91893853320467274178f;
+// One action's term of the Gaussian log-prob (AC:341-345), log_sg = logf(sg).  The PPO loss of both paths (c2_fin_ppo, ppo_loss_kernel) and
+// ppo_diag_kernel sum it over a channel's actions in index order, so the diagnostics see the ratio the loss saw, bit for bit.
+__device__ __forceinline__ float ppo_logp_term(float a, float mu, float sg, float log_sg) {
+  const float d = a - mu;
+  return -(d * d) / (2.0f * (sg * sg)) - log_sg - C2_LOG_SQRT_2PI;
+}
 
 // ---- fp32 pairs ---------------------------------------------------------------------------------------------------------
 // two fp32 values side by side in a 64-bit register, as a 16-byte load delivers them; the arithmetic is element-wise
@@ -340,9 +346,8 @@ __device__ __forceinline__ void c2_fin_ppo(const FinArgs& f, int c, int64_t m, b
 #pragma unroll
     for (int i = 0; i < C2_GRP; ++i) {
       if (i < cnt) {
-        const float d = act[i] - v[i];
         const float ls = logf(sg[i]);
-        lp += -(d * d) / (2.0f * (sg[i] * sg[i])) - ls - C2_LOG_SQRT_2PI;
+        lp += ppo_logp_term(act[i], v[i], sg[i], ls);
         l_ent += 0.5f + C2_LOG_SQRT_2PI + ls;
       }
     }

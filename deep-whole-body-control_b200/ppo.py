@@ -8,6 +8,7 @@ Every numerical step runs in libdwbc kernels; this class only sequences launches
   process_env_step -> dwbc_store_rewards (time-out bootstrap PPO:133-134) [+ dwbc_track_episodes, OPR:140-154]
   compute_returns  -> dwbc_critic_values + dwbc_gae
   update         -> per mini-batch: dwbc_ppo_minibatch_grad [+ NCCL all-reduce] + dwbc_clip_adam_step
+                    (diagnostics=True: dwbc_explained_variance once, dwbc_ppo_minibatch_grad_diag per mini-batch)
   update_dagger  -> per mini-batch: dwbc_dagger_minibatch_grad [+ all-reduce] + dwbc_clip_adam_step
 
 Host<->device synchronisation happens once per update (to return the mean losses), not three
@@ -81,7 +82,8 @@ class FusedPPO:
                  use_clipped_value_loss=True, schedule="fixed", desired_kl=0.01, device="cuda:0",
                  mixing_schedule=(0.5, 2000, 4000), torque_supervision=False, torque_supervision_schedule=(0.1, 1000, 1000),
                  adaptive_arm_gains=False, min_policy_std=None, dagger_update_freq=20, priv_reg_coef_schedual=(0, 0, 0, 1),
-                 world_size=1, process_group=None, precision="tf32x3", cuda_graphs=False, track_episodes=0):
+                 world_size=1, process_group=None, precision="tf32x3", cuda_graphs=False, track_episodes=0,
+                 diagnostics=False):
         if adaptive_arm_gains:
             raise L.DwbcError("adaptive_arm_gains (a 12-output arm head, AC:111-125,214-215; off for widowGo1, WGC:168) is not implemented")
         if schedule != "fixed":
@@ -133,6 +135,15 @@ class FusedPPO:
             raise L.DwbcError(f"track_episodes must be a non-negative int (the number of finished episodes kept), not {track_episodes!r}")
         self.track_episodes = track_episodes
         self._episodes = None
+        # diagnostics: update() also measures approximate KL, clip fractions, pre-clip gradient norms and explained variance on the device,
+        # captured with it; update_diagnostics() reads them once per call (DESIGN §13)
+        if not isinstance(diagnostics, bool):
+            raise L.DwbcError(f"diagnostics must be True or False, not {diagnostics!r}")
+        self.diagnostics = diagnostics
+        self._diag, self._diag_steps = None, 0          # [mini-batches, DIAG_N] of the last update(), and how many it ran
+        if diagnostics:
+            self._diag_ev = torch.zeros(2, device=self.device)                                  # explained variance (leg, arm)
+            self._ev_scratch = torch.zeros(L.EV_SCRATCH, dtype=torch.float64, device=self.device)
 
     # ------------------------------------------------------------------ plumbing
     def init_storage(self, num_envs, num_transitions_per_env, actor_obs_shape, critic_obs_shape, action_shape):
@@ -348,8 +359,16 @@ class FusedPPO:
         indices = indices.to(torch.int64).contiguous()
         mbs = indices.numel() // self.num_mini_batches
         ws = self._workspace(mbs)
+        self._diag_buffer()
         self._ppo_launches(hp, indices, mbs, ws, on_step)
         return self._ppo_finish(hp)
+
+    def _diag_buffer(self):
+        """The per-mini-batch diagnostics slots of one update() (diagnostics on), allocated for the current mini-batch count."""
+        n = self.num_learning_epochs * self.num_mini_batches
+        if self.diagnostics and (self._diag is None or self._diag.shape[0] != n):
+            self._diag = torch.zeros(n, L.DIAG_N, device=self.device)
+        return self._diag
 
     def _zh_buffer(self):
         s = self.storage
@@ -376,8 +395,17 @@ class FusedPPO:
             L.check(self._lib.dwbc_hist_latent(C.addressof(ac.net_cfg), L.ptr(ac.flat), L.ptr(obs_flat[r0:]), obs_flat.stride(0),
                                                L.ptr(zh[r0:]), lld, nrow, L.ptr(ws), L.stream_ptr()), "dwbc_hist_latent")
         s.set_hist_latent(zh)
+        diag = self._diag if self.diagnostics else None
+        if diag is not None:
+            L.check(self._lib.dwbc_explained_variance(L.ptr(s.values), L.ptr(s.returns), total, L.ptr(self._ev_scratch), L.ptr(self._diag_ev),
+                                                      L.stream_ptr()), "dwbc_explained_variance")
         for batch_idx in s.mini_batch_generator(self.num_mini_batches, self.num_learning_epochs, indices):
-            if dev is None:
+            if diag is not None:
+                L.check(self._lib.dwbc_ppo_minibatch_grad_diag(C.addressof(ac.net_cfg), L.ptr(ac.flat), s.c_struct_ptr(), L.ptr(batch_idx), mbs,
+                                                               C.addressof(hp), None if dev is None else dev[0], L.ptr(s.mu), L.ptr(s.sigma),
+                                                               L.ptr(self.grad), L.ptr(self._losses), L.ptr(diag[k]), L.ptr(ws), L.stream_ptr()),
+                        "dwbc_ppo_minibatch_grad_diag")
+            elif dev is None:
                 L.check(self._lib.dwbc_ppo_minibatch_grad(C.addressof(ac.net_cfg), L.ptr(ac.flat), s.c_struct_ptr(), L.ptr(batch_idx), mbs,
                                                           C.addressof(hp), L.ptr(self.grad), L.ptr(self._losses), L.ptr(ws), L.stream_ptr()),
                         "dwbc_ppo_minibatch_grad")
@@ -389,14 +417,15 @@ class FusedPPO:
             if on_step is not None:
                 on_step(k, "grad")
             opt = self.optimizer
+            norm_out = self._grad_norm if diag is None else diag[k, L.DIAG_GRAD_NORM:]       # the pre-clip norm of step k
             if dev is None:
                 opt.step += 1
                 L.check(self._lib.dwbc_clip_adam_step(L.ptr(ac.flat), L.ptr(self.grad), L.ptr(opt.m), L.ptr(opt.v), 0, ac.num_params,
-                                                      C.addressof(hp), opt.step, L.ptr(self._norm_scratch), L.ptr(self._grad_norm),
+                                                      C.addressof(hp), opt.step, L.ptr(self._norm_scratch), L.ptr(norm_out),
                                                       L.stream_ptr()), "dwbc_clip_adam_step")
             else:
                 L.check(self._lib.dwbc_clip_adam_step_table(L.ptr(ac.flat), L.ptr(self.grad), L.ptr(opt.m), L.ptr(opt.v), 0, ac.num_params,
-                                                            C.addressof(hp), k + 1, dev[1], L.ptr(self._norm_scratch), L.ptr(self._grad_norm),
+                                                            C.addressof(hp), k + 1, dev[1], L.ptr(self._norm_scratch), L.ptr(norm_out),
                                                             L.stream_ptr()), "dwbc_clip_adam_step_table")
             if on_step is not None:
                 on_step(k, "step")
@@ -408,12 +437,38 @@ class FusedPPO:
         num_updates = self.num_learning_epochs * self.num_mini_batches
         losses = (self._losses / num_updates).tolist()                                   # single sync per update
         s.clear()
+        if self.diagnostics:
+            self._diag_steps = num_updates
         value_mixing_ratio, priv_reg_coef = hp.mixing_ratio, hp.priv_reg_coef
         self.counter += 1                                                                 # PPO:259
         self.enforce_min_std()
         self.last_entropy = losses[3]
         ts_w = hp.torque_supervision_weight if self.torque_supervision else 0                            # PPO:158
         return losses[1], losses[0], (losses[4] if self.torque_supervision else 0.0), value_mixing_ratio, ts_w, losses[2], priv_reg_coef  # PPO:263
+
+    def update_diagnostics(self):
+        """Diagnostics of the last update() (FusedPPO(diagnostics=True)), read with one synchronisation: the means over its mini-batches
+        of approx_kl (= approx_kl_leg + approx_kl_arm, the KL rsl_rl's adaptive schedule computes, between the rollout policy and the
+        parameters each mini-batch saw), clip_fraction_leg / _arm (share of rows whose ratio the clip cut off), grad_norm (pre-clip) and
+        grad_norm_max, the value function's explained_variance_leg / _arm (1 - Var(R - V) / Var(R) over the storage, NaN where Var(R) = 0),
+        and under 'per_minibatch' the same per mini-batch, in update order.  With world_size > 1 the values are this rank's own (its rows,
+        its parameters; the gradient norm is of the all-reduced gradient).  Not training state: checkpoints do not include them."""
+        if not self.diagnostics:
+            raise L.DwbcError("update_diagnostics() needs FusedPPO(diagnostics=True)")
+        if not self._diag_steps:
+            raise L.DwbcError("update_diagnostics(): no update() has run yet")
+        d = self._diag.to("cpu", non_blocking=True)
+        ev = self._diag_ev.to("cpu", non_blocking=True)
+        if self.device.type == "cuda":
+            torch.cuda.current_stream(self.device).synchronize()
+        d = d.double()
+        per = dict(approx_kl=(d[:, L.DIAG_KL_LEG] + d[:, L.DIAG_KL_ARM]).tolist(), approx_kl_leg=d[:, L.DIAG_KL_LEG].tolist(),
+                   approx_kl_arm=d[:, L.DIAG_KL_ARM].tolist(), clip_fraction_leg=d[:, L.DIAG_CLIP_LEG].tolist(),
+                   clip_fraction_arm=d[:, L.DIAG_CLIP_ARM].tolist(), grad_norm=d[:, L.DIAG_GRAD_NORM].tolist())
+        out = {k: sum(v) / len(v) for k, v in per.items()}
+        out.update(grad_norm_max=max(per["grad_norm"]), explained_variance_leg=float(ev[0]), explained_variance_arm=float(ev[1]),
+                   per_minibatch=per)
+        return out
 
     def update_dagger(self, indices=None):
         """PPO:265-291."""
@@ -462,10 +517,13 @@ class FusedPPO:
         """What a captured update depends on beyond the per-iteration scalars: a change re-captures.  Storage shape and buffers,
         mini-batching, precision, network and workspace, torque supervision, and the hyper-parameters the launches carry by value."""
         s, ac, h = self.storage, self.actor_critic, self._hp
-        return (kind, s.num_transitions_per_env, s.num_envs, s._obs_all.data_ptr(), self.num_mini_batches, self.num_learning_epochs,
-                self._precision, ac.flat.data_ptr(), bytes(ac.net_cfg), self._ws.data_ptr(), self._ws_rows, self.torque_supervision,
-                h.clip_param, h.value_loss_coef, h.entropy_coef, h.use_clipped_value_loss, h.max_grad_norm, h.lr, h.beta1, h.beta2,
-                h.adam_eps, h.grad_scale, h.arm_coefs)
+        key = (kind, s.num_transitions_per_env, s.num_envs, s._obs_all.data_ptr(), self.num_mini_batches, self.num_learning_epochs,
+               self._precision, ac.flat.data_ptr(), bytes(ac.net_cfg), self._ws.data_ptr(), self._ws_rows, self.torque_supervision,
+               h.clip_param, h.value_loss_coef, h.entropy_coef, h.use_clipped_value_loss, h.max_grad_norm, h.lr, h.beta1, h.beta2,
+               h.adam_eps, h.grad_scale, h.arm_coefs)
+        if self.diagnostics and kind == "ppo":
+            key += (("diagnostics", self._diag_buffer().data_ptr()),)
+        return key
 
     def _update_graphed(self, kind, indices):
         """update() / update_dagger() as one CUDA graph: captured on the first call for a key (graph_key), replayed on later calls.  The
@@ -483,6 +541,7 @@ class FusedPPO:
         self._workspace(mbs)
         if kind == "ppo":
             self._zh_buffer()
+            self._diag_buffer()
         n_steps = self.num_learning_epochs * self.num_mini_batches
         key = self.graph_key(kind) + (indices.numel(),)
         g = self._graphs.get(kind)

@@ -413,6 +413,35 @@ int dwbc_ppo_minibatch_grad_sched(const DwbcNetCfg* net, const float* params, co
                                   int32_t M, const DwbcPpoHyper* hp, const float* sched, float* grad, float* losses_out, void* workspace,
                                   dwbc_stream_t stream);
 
+/* Diagnostics of one PPO mini-batch: diag_out[DWBC_DIAG_N] (fp32, device).  Per channel c (leg = the first n_leg actions, arm = the rest),
+ * over the M gathered rows, with mu_new the forward's action means, sigma_new the std parameters it used (before the Adam step), and
+ * mu_old / sigma_old the rows' rollout means and sigmas:
+ *   KL_c   = mean_rows sum_{i in c} log(sigma_new / sigma_old + 1e-5) + (sigma_old^2 + (mu_old - mu_new)^2) / (2 sigma_new^2) - 0.5
+ *            (the KL rsl_rl's adaptive learning-rate schedule computes; evaluated in double, the total is LEG + ARM)
+ *   CLIP_c = share of rows whose ratio exp(logp_new - logp_old) lies outside [1 - clip, 1 + clip]: the ratio the loss computed, bit for bit
+ *   GRAD_NORM: not written by the mini-batch call; pass diag_out + DWBC_DIAG_GRAD_NORM as grad_norm_out of dwbc_clip_adam_step(_table)
+ *            to keep that step's pre-clip gradient norm there.
+ * Every mean is a fixed-order sum (one partial per 128-row block, added in block order): bitwise repeatable. */
+#define DWBC_DIAG_KL_LEG 0
+#define DWBC_DIAG_KL_ARM 1
+#define DWBC_DIAG_CLIP_LEG 2
+#define DWBC_DIAG_CLIP_ARM 3
+#define DWBC_DIAG_GRAD_NORM 4
+#define DWBC_DIAG_N 5
+/* dwbc_ppo_minibatch_grad (sched == NULL) or dwbc_ppo_minibatch_grad_sched (sched != NULL), with the same launches and the same results in
+ * grad and losses_out, plus the diagnostics of the mini-batch in diag_out[DWBC_DIAG_KL_LEG .. DWBC_DIAG_CLIP_ARM] (overwritten).
+ * old_mu, old_sigma: [T*N, n_leg + n_arm] rollout storage rows (RS:71-72), gathered through idx like the others.  NULL old_mu, old_sigma
+ * or diag_out: DWBC_ERR_ARG. */
+int dwbc_ppo_minibatch_grad_diag(const DwbcNetCfg* net, const float* params, const DwbcStorage* st, const int64_t* idx, int32_t M,
+                                 const DwbcPpoHyper* hp, const float* sched, const float* old_mu, const float* old_sigma, float* grad,
+                                 float* losses_out, float* diag_out, void* workspace, dwbc_stream_t stream);
+/* Explained variance of the value function per channel, out[2] (fp32, device) = 1 - Var(R - V) / Var(R) over rows x 2 values / returns
+ * (population variances; NaN where Var(R) == 0).  Sums in double, one partial per block added in block order by the last block: bitwise
+ * repeatable.  scratch[DWBC_EV_SCRATCH] (double) is device scratch the caller zeroes once; every call leaves its counter at zero. */
+#define DWBC_EV_MAX_BLOCKS 256
+#define DWBC_EV_SCRATCH (2 + 8 * DWBC_EV_MAX_BLOCKS)
+int dwbc_explained_variance(const float* values, const float* returns, int64_t rows, double* scratch, float* out, dwbc_stream_t stream);
+
 /* PPO.update_dagger mini-batch (PPO:273-283): grad of mean ||sg(z_priv) - z_hist||_2 w.r.t. the
  * history-encoder parameters only (other entries of grad are zeroed). losses_out[0] += loss. */
 int dwbc_dagger_minibatch_grad(const DwbcNetCfg* net, const float* params, const DwbcStorage* st, const int64_t* idx,

@@ -19,7 +19,8 @@ int dwbc_debug_gemm(int mode, int tc, const float* A, int64_t lda, const float* 
 int dwbc_debug_set_tc_cycle_buffer(unsigned long long* dev_ptr);
 
 /* The chain programs a call would launch, described without launching (host code, no GPU).  what: 0 = dwbc_policy_act, 1 = dwbc_critic_values,
- * 2 / 3 = forward + loss / backward launch of dwbc_ppo_minibatch_grad, 4 = dwbc_policy_mean (on networks dwbc_policy_act runs on the chains).  out = [nprog, pack items, per program: n_ops, n_loads, per op: N, kpad,
+ * 2 / 3 = forward + loss / backward launch of dwbc_ppo_minibatch_grad, 4 = dwbc_policy_mean (on networks dwbc_policy_act runs on the chains),
+ * 5 = forward + loss of dwbc_ppo_minibatch_grad_diag (2 with the heads' means written for the diagnostics).  out = [nprog, pack items, per program: n_ops, n_loads, per op: N, kpad,
  * act, fin, fin_c, out_col0, has_global_output, output_is_tile_image]; returns the number of ints written or a negative DWBC_ERR_*. */
 int dwbc_debug_describe_chain(const DwbcNetCfg* net, int32_t rows, int what, int hist_encoding, int sms, int32_t* out, int32_t out_len);
 /* the work-item planner of the fused chain kernel (mlp_chain2.cuh) on its own (host code, no GPU): items per program and simulated
