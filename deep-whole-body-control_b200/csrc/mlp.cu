@@ -531,149 +531,105 @@ static int build_forward(const DwbcNetCfg& n, const float* P, const float* obs, 
   return DWBC_OK;
 }
 
-// ---- rollout sampling + log-prob (AC:326-345, PPO:119-123) -------------------------------------
-constexpr float LOG_SQRT_2PI = 0.91893853320467274178f;
-
-__global__ void act_finalize_kernel(const float* __restrict__ mean_in, int mean_ld, const float* __restrict__ std, const float* __restrict__ eps,
-                                    float* __restrict__ actions, float* __restrict__ log_prob, float* __restrict__ mean_out,
-                                    float* __restrict__ sigma_out, int rows, int n_leg, int n_act) {
+// ---- rollout sampling + log-prob (AC:326-345, PPO:119-123) of the forward's means [rows, mean_ld] -------------
+__global__ void act_finalize_kernel(const FinArgs f, const float* __restrict__ mean_in, int mean_ld) {
   int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= rows) return;
+  if (r >= f.rows) return;
   float lp[2] = {0.0f, 0.0f};
-  for (int i = 0; i < n_act; ++i) {
-    const float mu = mean_in[(int64_t)r * mean_ld + i], sg = std[i];
-    const float a = mu + sg * eps[(int64_t)r * n_act + i];
-    const float d = a - mu;
-    lp[i < n_leg ? 0 : 1] += -(d * d) / (2.0f * (sg * sg)) - logf(sg) - LOG_SQRT_2PI;
-    actions[(int64_t)r * n_act + i] = a;
-    mean_out[(int64_t)r * n_act + i] = mu;
-    sigma_out[(int64_t)r * n_act + i] = sg;
+  for (int i = 0; i < f.n_act; ++i) {
+    const float mu = mean_in[(int64_t)r * mean_ld + i], sg = f.std[i];
+    const float a = mu + sg * f.eps[(int64_t)r * f.n_act + i];
+    lp[i < f.n_leg ? 0 : 1] += ppo_logp_term(a, mu, sg, logf(sg));
+    f.actions[(int64_t)r * f.n_act + i] = a;
+    f.mean_out[(int64_t)r * f.n_act + i] = mu;
+    f.sigma_out[(int64_t)r * f.n_act + i] = sg;
   }
-  log_prob[2 * r] = lp[0];
-  log_prob[2 * r + 1] = lp[1];
+  f.log_prob[2 * r] = lp[0];
+  f.log_prob[2 * r + 1] = lp[1];
 }
 
 // ---- PPO loss and its derivative w.r.t. the network outputs (PPO:166-221) ----------------------
-struct LossArgs {
-  const float* mean; int mean_ld; const float* std; const float* value; const float* zp; int zld; const float* zh; int64_t zh_ld; int zh_by_src;
-  const float* actions; const float* old_logp; const float* old_values; const float* returns; const float* adv; const int64_t* idx;
-  float* g_leg; int gleg_ld; float* g_arm; int garm_ld; float* g_vl; float* g_va; int gv_ld; float* g_z;
-  float* grad_std; float* losses;
-  float* part; unsigned* ticket;          // [blocks][LOSS_PART] partials, added up in block order by the last block
-  int rows, n_leg, n_act, latent;
-  float clip, c_value, c_ent, c_reg, rho;
-  int clipped_value;
-  const float* ts_target; const float* ts_pos; const float* ts_vel; const float* ts_coef; float ts_w;      // arm torque supervision (PPO:224-239)
-  const float* sched;                     // optional device (c_reg, rho, ts_w) in place of the three fields (dwbc_ppo_minibatch_grad_sched)
-};
-
-__global__ void __launch_bounds__(128) ppo_loss_kernel(const LossArgs a) {
+// The forward's outputs: means [rows, mean_ld], values [rows, 2], privileged latent zp [rows, f.gz_ld].  f.part: [blocks][LOSS_PART]
+// partials, added up in block order by the last block (ticket).
+__global__ void __launch_bounds__(128) ppo_loss_kernel(const FinArgs f, const float* mean, int mean_ld, const float* value, const float* zp,
+                                                       unsigned* ticket) {
   __shared__ float red[5 + 32][4];
   __shared__ float sched_s[3];            // the schedule values, loaded once per CTA
   if (threadIdx.x == 0) {
-    sched_s[0] = a.sched ? a.sched[0] : a.c_reg;
-    sched_s[1] = a.sched ? a.sched[1] : a.rho;
-    sched_s[2] = a.sched ? a.sched[2] : a.ts_w;
+    sched_s[0] = f.sched ? f.sched[0] : f.c_reg;
+    sched_s[1] = f.sched ? f.sched[1] : f.rho;
+    sched_s[2] = f.sched ? f.sched[2] : f.ts_w;
   }
   __syncthreads();
   const float c_reg = sched_s[0], rho = sched_s[1], ts_w = sched_s[2];
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
-  const bool on = r < a.rows;
-  const float inv2m = 1.0f / (2.0f * (float)a.rows), invm = 1.0f / (float)a.rows;
+  const bool on = r < f.rows;
+  const float inv2m = 1.0f / (2.0f * (float)f.rows), invm = 1.0f / (float)f.rows;
   float l_surr = 0.0f, l_val = 0.0f, l_reg = 0.0f, l_ent = 0.0f, l_ts = 0.0f;
   float gstd[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) gstd[i] = 0.0f;
   if (on) {
-    const int64_t src = a.idx ? a.idx[r] : r;
-    const float* mu = a.mean + (int64_t)r * a.mean_ld;
-    const float* act = a.actions + src * a.n_act;
+    const int64_t src = f.idx ? f.idx[r] : r;
+    const float* mu = mean + (int64_t)r * mean_ld;
+    const float* act = f.s_actions + src * f.n_act;
     float lp[2] = {0.0f, 0.0f}, ent[2] = {0.0f, 0.0f};
-    for (int i = 0; i < a.n_act; ++i) {
-      const float sg = a.std[i];
-      const int c = i < a.n_leg ? 0 : 1;
-      lp[c] += ppo_logp_term(act[i], mu[i], sg, logf(sg));                        // AC:341-345
-      ent[c] += 0.5f + LOG_SQRT_2PI + logf(sg);                                  // AC:326-331 (0.5 log 2pi == log sqrt 2pi)
+    for (int i = 0; i < f.n_act; ++i) {
+      const float sg = f.std[i];
+      const int c = i < f.n_leg ? 0 : 1;
+      lp[c] += ppo_logp_term(act[i], mu[i], sg, logf(sg));
+      ent[c] += ppo_entropy_term(logf(sg));
     }
-    const float a0 = a.adv[2 * src], a1 = a.adv[2 * src + 1];
-    const float mix[2] = {a0 + rho * a1, a1 + rho * a0};                           // PPO:199-201
+    const float2 adv = make_float2(f.adv[2 * src], f.adv[2 * src + 1]);
     float glp[2];
 #pragma unroll
     for (int c = 0; c < 2; ++c) {
-      const float ratio = expf(lp[c] - a.old_logp[2 * src + c]);                   // PPO:202
-      const float rc = fminf(fmaxf(ratio, 1.0f - a.clip), 1.0f + a.clip);
-      const float s1 = -mix[c] * ratio, s2 = -mix[c] * rc;                         // PPO:203-205
-      l_surr += fmaxf(s1, s2);
-      const bool inside = ratio >= 1.0f - a.clip && ratio <= 1.0f + a.clip;
-      float g = 0.0f;                                                              // d max(s1,s2) / d ratio
-      if (s1 > s2) g = -mix[c];
-      else if (s1 == s2) g = 0.5f * -mix[c] + (inside ? 0.5f * -mix[c] : 0.0f);
-      else g = inside ? -mix[c] : 0.0f;
-      glp[c] = inv2m * g * ratio;
+      const float ratio = ppo_ratio(lp[c], f.old_logp[2 * src + c]);
+      const float2 surr = ppo_surrogate(ppo_mix(adv, c, rho), ratio, f.clip);
+      l_surr += surr.x;
+      glp[c] = inv2m * surr.y * ratio;
       l_ent += ent[c];
     }
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
-      if (i < a.n_act) {
-        const float sg = a.std[i], d = act[i] - mu[i];
-        const int c = i < a.n_leg ? 0 : 1;
-        float gmu = glp[c] * d / (sg * sg) * (1.0f - mu[i] * mu[i]);               // through tanh (AC:157,170)
-        if (c == 1 && a.ts_target != nullptr) {
-          // arm torque supervision: tau = kp (mu + q_default - q) - kd qd (PPO:318-323), loss w * mean((tau - target)^2) (PPO:236-238)
-          const int n_arm = a.n_act - a.n_leg, j = i - a.n_leg;
-          const float kp = a.ts_coef[j];
-          const float e = kp * (mu[i] + a.ts_coef[2 * n_arm + j] - a.ts_pos[src * n_arm + j]) - a.ts_coef[n_arm + j] * a.ts_vel[src * n_arm + j] -
-                          a.ts_target[src * n_arm + j];
-          l_ts += e * e;
-          gmu += 2.0f * ts_w / ((float)a.rows * (float)n_arm) * e * kp * (1.0f - mu[i] * mu[i]);
+      if (i < f.n_act) {
+        const float sg = f.std[i], ai = act[i], mi = mu[i];      // loaded once: the compiler cannot rule out that the stores below alias them
+        const int c = i < f.n_leg ? 0 : 1;
+        float gmu = ppo_grad_mean(glp[c], ai, mi, sg);
+        if (c == 1 && f.ts_target != nullptr) {
+          const float2 t = ppo_torque_term(f, src, f.n_act - f.n_leg, i - f.n_leg, mi, ts_w);
+          l_ts += t.x;
+          gmu += t.y;
         }
-        if (c == 0) a.g_leg[(int64_t)r * a.gleg_ld + i] = gmu;
-        else a.g_arm[(int64_t)r * a.garm_ld + (i - a.n_leg)] = gmu;
-        gstd[i] = glp[c] * ((d * d) / (sg * sg * sg) - 1.0f / sg) - a.c_ent * inv2m / sg;
+        if (c == 0) f.g_leg[(int64_t)r * f.gleg_ld + i] = gmu;
+        else f.g_arm[(int64_t)r * f.garm_ld + (i - f.n_leg)] = gmu;
+        gstd[i] = ppo_grad_std(glp[c], ai, mi, sg, f.c_ent, inv2m);
       }
     }
-    // value loss PPO:209-216
     float gv[2];
 #pragma unroll
     for (int c = 0; c < 2; ++c) {
-      const float v = a.value[2 * r + c], vo = a.old_values[2 * src + c], R = a.returns[2 * src + c];
-      const float l1 = (v - R) * (v - R);
-      if (a.clipped_value) {
-        const float dvo = v - vo;
-        const float vc = vo + fminf(fmaxf(dvo, -a.clip), a.clip);
-        const float l2 = (vc - R) * (vc - R);
-        const bool inside = dvo >= -a.clip && dvo <= a.clip;
-        l_val += fmaxf(l1, l2);
-        const float g1 = 2.0f * (v - R), g2 = inside ? 2.0f * (vc - R) : 0.0f;
-        gv[c] = l1 > l2 ? g1 : (l1 == l2 ? 0.5f * g1 + 0.5f * g2 : g2);
-      } else {
-        l_val += l1;
-        gv[c] = 2.0f * (v - R);
-      }
-      gv[c] *= a.c_value * inv2m;
+      const float2 t = ppo_value_term(value[2 * r + c], f.old_values[2 * src + c], f.returns[2 * src + c], f.clip, f.clipped_value);
+      l_val += t.x;
+      gv[c] = t.y * (f.c_value * inv2m);
     }
-    a.g_vl[(int64_t)r * a.gv_ld] = gv[0];
-    a.g_va[(int64_t)r * a.gv_ld] = gv[1];
+    f.g_v[(int64_t)r * f.gv_ld] = gv[0];
+    f.g_v[(int64_t)r * f.gv_ld + 1] = gv[1];
     // pad columns are read as (zero-weighted) operand columns by the tensor-core backward: keep them finite
-    for (int i = 2; i < a.gv_ld; ++i) a.g_vl[(int64_t)r * a.gv_ld + i] = 0.0f;
-    for (int i = a.n_leg; i < a.gleg_ld; ++i) a.g_leg[(int64_t)r * a.gleg_ld + i] = 0.0f;
-    for (int i = a.n_act - a.n_leg; i < a.garm_ld; ++i) a.g_arm[(int64_t)r * a.garm_ld + i] = 0.0f;
-    // privileged-latent regulariser PPO:174-177
-    float nrm = 0.0f;
-    const float* zhr = a.zh + (a.zh_by_src ? src : (int64_t)r) * a.zh_ld;     // precomputed per storage row, or per mini-batch row
-    for (int i = 0; i < a.latent; ++i) {
-      const float d = a.zp[(int64_t)r * a.zld + i] - zhr[i];
-      nrm += d * d;
-    }
-    nrm = sqrtf(nrm);
+    for (int i = 2; i < f.gv_ld; ++i) f.g_v[(int64_t)r * f.gv_ld + i] = 0.0f;
+    for (int i = f.n_leg; i < f.gleg_ld; ++i) f.g_leg[(int64_t)r * f.gleg_ld + i] = 0.0f;
+    for (int i = f.n_act - f.n_leg; i < f.garm_ld; ++i) f.g_arm[(int64_t)r * f.garm_ld + i] = 0.0f;
+    const float* zpr = zp + (int64_t)r * f.gz_ld;
+    const float* zhr = f.zh + (f.zh_by_src ? src : (int64_t)r) * f.zh_ld;     // precomputed per storage row, or per mini-batch row
+    const float nrm = ppo_reg_norm<0>(zpr, zhr, f.latent);
     l_reg = nrm;
-    const float s = nrm > 0.0f ? c_reg * invm / nrm : 0.0f;
-    for (int i = 0; i < a.latent; ++i)
-      a.g_z[(int64_t)r * a.zld + i] = s * (a.zp[(int64_t)r * a.zld + i] - zhr[i]);
+    const float s = ppo_reg_scale(nrm, c_reg, invm);
+    for (int i = 0; i < f.latent; ++i)
+      f.g_z[(int64_t)r * f.gz_ld + i] = s * (zpr[i] - zhr[i]);
   }
   // warp sums -> this block's slot; the last block adds the slots up in block order
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  float v4[5] = {l_surr * inv2m, l_val * inv2m, l_reg * invm, l_ent * inv2m, l_ts * invm / (float)max(a.n_act - a.n_leg, 1)};
+  float v4[5] = {l_surr * inv2m, l_val * inv2m, l_reg * invm, l_ent * inv2m, l_ts * invm / (float)max(f.n_act - f.n_leg, 1)};
 #pragma unroll
   for (int k = 0; k < 5; ++k) {
     float s = warp_sum(v4[k]);
@@ -681,19 +637,19 @@ __global__ void __launch_bounds__(128) ppo_loss_kernel(const LossArgs a) {
   }
 #pragma unroll
   for (int i = 0; i < 32; ++i) {
-    if (i < a.n_act) {
+    if (i < f.n_act) {
       float s = warp_sum(gstd[i]);
       if (lane == 0) red[5 + i][w] = s;
     }
   }
   __syncthreads();
-  const int nq = 5 + a.n_act, q = threadIdx.x;
-  if (q < nq) a.part[(int64_t)blockIdx.x * LOSS_PART + q] = (red[q][0] + red[q][1]) + (red[q][2] + red[q][3]);
-  if (!last_block(a.ticket) || q >= nq) return;
+  const int nq = 5 + f.n_act, q = threadIdx.x;
+  if (q < nq) f.part[(int64_t)blockIdx.x * LOSS_PART + q] = (red[q][0] + red[q][1]) + (red[q][2] + red[q][3]);
+  if (!last_block(ticket) || q >= nq) return;
   float s = 0.0f;
-  for (int b = 0; b < (int)gridDim.x; ++b) s += __ldcg(a.part + (int64_t)b * LOSS_PART + q);
-  if (q >= 5) a.grad_std[q - 5] += s;
-  else if (q < 4 || a.ts_target != nullptr) a.losses[q] += s;
+  for (int b = 0; b < (int)gridDim.x; ++b) s += __ldcg(f.part + (int64_t)b * LOSS_PART + q);
+  if (q >= 5) f.grad_std[q - 5] += s;
+  else if (q < 4 || f.ts_target != nullptr) f.losses[q] += s;
 }
 
 // DAgger loss PPO:273-276: mean_rows || sg(zp) - zh ||_2 ; writes d/d zh_pre (the derivative of the activation `act` folded in)
@@ -704,12 +660,7 @@ __global__ void __launch_bounds__(128) dagger_loss_kernel(const float* __restric
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   float l = 0.0f;
   if (r < rows) {
-    float nrm = 0.0f;
-    for (int i = 0; i < latent; ++i) {
-      const float d = zp[(int64_t)r * zld + i] - zh[(int64_t)r * zld + i];
-      nrm += d * d;
-    }
-    nrm = sqrtf(nrm);
+    const float nrm = ppo_reg_norm<0>(zp + (int64_t)r * zld, zh + (int64_t)r * zld, latent);
     l = nrm / (float)rows;
     const float s = nrm > 0.0f ? 1.0f / ((float)rows * nrm) : 0.0f;
     for (int i = 0; i < latent; ++i) {
@@ -731,8 +682,9 @@ __global__ void __launch_bounds__(128) dagger_loss_kernel(const float* __restric
 // Per channel c (leg = actions [0, n_leg), arm = the rest), over the M rows of a mini-batch:
 //   approx_kl[c]     = mean_rows sum_i log(sg_new / sg_old + 1e-5) + (sg_old^2 + (mu_old - mu_new)^2) / (2 sg_new^2) - 0.5  (rsl_rl's KL)
 //   clip_fraction[c] = share of rows whose ratio lies outside [1 - clip, 1 + clip]
-// The ratio is the loss's: ppo_logp_term summed in index order over the same new means, std and stored rows.  The KL terms are evaluated
-// and summed in double.  One partial per 128-row block, added up in block order by the last block.
+// The ratio is the loss's: ppo_logp_term summed in index order over the same new means, std and stored rows, and the loss's ratio and
+// clip-range test (ppo_terms.cuh).  The KL terms are evaluated and summed in double.  One partial per 128-row block, added up in block order
+// by the last block.
 static_assert(DWBC_DIAG_KL_ARM == DWBC_DIAG_KL_LEG + 1 && DWBC_DIAG_CLIP_LEG == DWBC_DIAG_KL_LEG + 2 && DWBC_DIAG_CLIP_ARM == DWBC_DIAG_KL_LEG + 3,
               "ppo_diag_kernel writes its four means to consecutive slots");
 struct DiagArgs {
@@ -764,10 +716,7 @@ __global__ void __launch_bounds__(128) ppo_diag_kernel(const DiagArgs a) {
       v[c] += log(sn / so + 1e-5) + (so * so + dm * dm) / (2.0 * sn * sn) - 0.5;
     }
 #pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      const float ratio = expf(lp[c] - a.old_logp[2 * src + c]);
-      v[2 + c] = (ratio >= 1.0f - a.clip && ratio <= 1.0f + a.clip) ? 0.0 : 1.0;
-    }
+    for (int c = 0; c < 2; ++c) v[2 + c] = ppo_inside(ppo_ratio(lp[c], a.old_logp[2 * src + c]), a.clip) ? 0.0 : 1.0;
   }
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
 #pragma unroll
@@ -989,11 +938,31 @@ extern "C" int64_t dwbc_workspace_bytes(const DwbcNetCfg* net, int64_t rows) {
   return make_plan(*net, rows, nullptr).bytes;
 }
 
-// FinArgs of the rollout hooks
+// FinArgs of the rollout hooks and of act_finalize_kernel
 static FinArgs fin_rollout(const DwbcNetCfg& n, const float* P, const float* eps, float* actions, float* log_prob, float* mean, float* sigma, int rows) {
   FinArgs f{};
   f.std = P + n.off_std; f.eps = eps; f.actions = actions; f.log_prob = log_prob; f.mean_out = mean; f.sigma_out = sigma;
   f.n_leg = n.n_leg; f.n_act = n.n_leg + n.n_arm; f.rows = rows;
+  return f;
+}
+
+// FinArgs of the update: the hooks of the forward chains and ppo_loss_kernel.  The loss gradients go to the workspace (g_v: [rows, 4],
+// the two value columns, then padding), the privileged latent's at the padded latent stride.
+static FinArgs fin_update(const DwbcNetCfg& n, const float* P, const DwbcStorage* s, const int64_t* idx, const DwbcPpoHyper* hp, const float* sched,
+                          const Plan& p, float* grad, float* losses, int rows) {
+  const int Lld = (int)align_up(p.latent, 4);
+  FinArgs f{};
+  f.std = P + n.off_std; f.idx = idx; f.s_actions = s->actions; f.old_logp = s->log_prob; f.old_values = s->values; f.returns = s->returns;
+  f.adv = s->advantages;
+  f.zh = s->hist_latent ? s->hist_latent : p.zh; f.zh_ld = s->hist_latent ? s->hist_latent_ld : Lld; f.zh_by_src = s->hist_latent ? 1 : 0;
+  f.g_leg = p.g_leg; f.gleg_ld = (int)align_up(n.n_leg, 4); f.g_arm = p.g_arm; f.garm_ld = (int)align_up(n.n_arm, 4);
+  f.g_v = p.g_vl; f.gv_ld = 4; f.g_z = p.g_z; f.gz_ld = Lld;
+  f.grad_std = grad + n.off_std; f.losses = losses; f.part = p.loss_part;
+  f.n_leg = n.n_leg; f.n_act = n.n_leg + n.n_arm; f.latent = p.latent; f.rows = rows;
+  f.clip = hp->clip_param; f.c_value = hp->value_loss_coef; f.c_ent = hp->entropy_coef; f.c_reg = hp->priv_reg_coef; f.rho = hp->mixing_ratio;
+  f.clipped_value = hp->use_clipped_value_loss;
+  f.ts_target = s->target_arm_torques; f.ts_pos = s->current_arm_dof_pos; f.ts_vel = s->current_arm_dof_vel; f.ts_coef = hp->arm_coefs;
+  f.ts_w = hp->torque_supervision_weight; f.sched = sched;
   return f;
 }
 
@@ -1024,8 +993,7 @@ extern "C" int dwbc_policy_act(const DwbcNetCfg* net, const float* params, const
   }
   TRY(actor_forward(n, params, obs, nullptr, obs_stride, rows, z, zld, p, st));
   TRY(critic_forward(n, params, obs, nullptr, obs_stride, rows, p, values, st));
-  act_finalize_kernel<<<(rows + 127) / 128, 128, 0, st>>>(p.mean, p.mean_ld, params + n.off_std, eps, actions, log_prob, mean, sigma, rows,
-                                                           n.n_leg, n.n_leg + n.n_arm);
+  act_finalize_kernel<<<(rows + 127) / 128, 128, 0, st>>>(fin_rollout(n, params, eps, actions, log_prob, mean, sigma, rows), p.mean, p.mean_ld);
   DWBC_LAUNCH_CHECK();
   return DWBC_OK;
 }
@@ -1109,7 +1077,6 @@ static int ppo_minibatch_grad(const DwbcNetCfg* net, const float* params, const 
   const int rows = M;
   Plan p = make_plan(n, rows, workspace);
   const int Lld = (int)align_up(p.latent, 4);
-  const int gleg_ld = (int)align_up(n.n_leg, 4), garm_ld = (int)align_up(n.n_arm, 4);
   // tensor-core path: forward chains with the loss in the heads' epilogues, backward chains, grouped weight gradients.  The weight images
   // of all four programs are packed by ONE launch (the parameters are constant within a mini-batch).
   const bool x3 = mlp_precision == 2;
@@ -1139,18 +1106,8 @@ static int ppo_minibatch_grad(const DwbcNetCfg* net, const float* params, const 
   // PPO:166,174,230; identical values, so each is evaluated once here)
   float* z = p.priv[n.n_priv_layers - 1];
   if (!s->hist_latent) TRY(hist_latent_only(n, P, s->observations, idx, s->obs_stride, rows, p, p.zh, Lld, st));           // PPO:175-176 (no grad)
+  const FinArgs f = fin_update(n, P, s, idx, hp, sched, p, grad, losses_out, rows);
   if (chains) {
-    FinArgs f{};
-    f.std = P + n.off_std; f.idx = idx; f.s_actions = s->actions; f.old_logp = s->log_prob; f.old_values = s->values; f.returns = s->returns;
-    f.adv = s->advantages;
-    f.zh = s->hist_latent ? s->hist_latent : p.zh; f.zh_ld = s->hist_latent ? s->hist_latent_ld : Lld; f.zh_by_src = s->hist_latent ? 1 : 0;
-    f.g_leg = p.g_leg; f.gleg_ld = gleg_ld; f.g_arm = p.g_arm; f.garm_ld = garm_ld; f.g_v = p.g_vl; f.gv_ld = 4; f.g_z = p.g_z; f.gz_ld = Lld;
-    f.grad_std = grad + n.off_std; f.losses = losses_out; f.part = p.loss_part;
-    f.n_leg = n.n_leg; f.n_act = n.n_leg + n.n_arm; f.latent = p.latent; f.rows = rows;
-    f.clip = hp->clip_param; f.c_value = hp->value_loss_coef; f.c_ent = hp->entropy_coef; f.c_reg = hp->priv_reg_coef; f.rho = hp->mixing_ratio;
-    f.clipped_value = hp->use_clipped_value_loss;
-    f.ts_target = s->target_arm_torques; f.ts_pos = s->current_arm_dof_pos; f.ts_vel = s->current_arm_dof_vel; f.ts_coef = hp->arm_coefs;
-    f.ts_w = hp->torque_supervision_weight; f.sched = sched;
     TRY(launch_pack2(ch.pl, st));
     TRY(launch_chain2(&ch.b[0].pr, &ch.b[1].pr, f, x3, p.queue, st));
     TRY(diag(n.n_leg + n.n_arm));
@@ -1161,17 +1118,7 @@ static int ppo_minibatch_grad(const DwbcNetCfg* net, const float* params, const 
   TRY(actor_forward(n, P, s->observations, idx, s->obs_stride, rows, z, Lld, p, st));
   TRY(critic_forward(n, P, s->observations, idx, s->obs_stride, rows, p, p.value, st));
 
-  LossArgs a{};
-  a.mean = p.mean; a.mean_ld = p.mean_ld; a.std = P + n.off_std; a.value = p.value; a.zp = z; a.zld = Lld; a.zh = s->hist_latent ? s->hist_latent : p.zh; a.zh_ld = s->hist_latent ? s->hist_latent_ld : Lld; a.zh_by_src = s->hist_latent ? 1 : 0;
-  a.actions = s->actions; a.old_logp = s->log_prob; a.old_values = s->values; a.returns = s->returns; a.adv = s->advantages; a.idx = idx;
-  a.g_leg = p.g_leg; a.gleg_ld = gleg_ld; a.g_arm = p.g_arm; a.garm_ld = garm_ld; a.g_vl = p.g_vl; a.g_va = p.g_va; a.gv_ld = 4; a.g_z = p.g_z;
-  a.grad_std = grad + n.off_std; a.losses = losses_out; a.part = p.loss_part; a.ticket = reinterpret_cast<unsigned*>(p.queue + 2);
-  a.rows = rows; a.n_leg = n.n_leg; a.n_act = n.n_leg + n.n_arm; a.latent = p.latent;
-  a.clip = hp->clip_param; a.c_value = hp->value_loss_coef; a.c_ent = hp->entropy_coef; a.c_reg = hp->priv_reg_coef; a.rho = hp->mixing_ratio;
-  a.clipped_value = hp->use_clipped_value_loss;
-  a.ts_target = s->target_arm_torques; a.ts_pos = s->current_arm_dof_pos; a.ts_vel = s->current_arm_dof_vel; a.ts_coef = hp->arm_coefs;
-  a.ts_w = hp->torque_supervision_weight; a.sched = sched;
-  ppo_loss_kernel<<<(rows + 127) / 128, 128, 0, st>>>(a);
+  ppo_loss_kernel<<<(rows + 127) / 128, 128, 0, st>>>(f, p.mean, p.mean_ld, p.value, z, reinterpret_cast<unsigned*>(p.queue + 2));
   DWBC_LAUNCH_CHECK();
   TRY(diag(p.mean_ld));
 
@@ -1201,9 +1148,9 @@ static int ppo_minibatch_grad(const DwbcNetCfg* net, const float* params, const 
   {
     const int nb = n.n_actor_layers, tdim = n.actor_dims[nb - 1];
     RowMat trunk = rowmat(p.ab[nb - 1], tdim);
-    TRY(head_backward(P, grad, rowmat(p.g_leg, gleg_ld), n.n_leg, n.n_leg_layers, n.leg_dims, n.off_aleg_w, n.off_aleg_b, p.al, trunk, tdim,
+    TRY(head_backward(P, grad, rowmat(p.g_leg, f.gleg_ld), n.n_leg, n.n_leg_layers, n.leg_dims, n.off_aleg_w, n.off_aleg_b, p.al, trunk, tdim,
                       p.d2, 0, 0, p.d0, p.d1, rows, st));
-    TRY(head_backward(P, grad, rowmat(p.g_arm, garm_ld), n.n_arm, n.n_arm_layers, n.arm_dims, n.off_aarm_w, n.off_aarm_b, p.aa, trunk, tdim,
+    TRY(head_backward(P, grad, rowmat(p.g_arm, f.garm_ld), n.n_arm, n.n_arm_layers, n.arm_dims, n.off_aarm_w, n.off_aarm_b, p.aa, trunk, tdim,
                       p.d2, 1, 1, p.d0, p.d1, rows, st));
     RowMat G = rowmat(p.d2, tdim);
     int gout = tdim;

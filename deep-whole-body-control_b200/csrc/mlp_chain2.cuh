@@ -32,6 +32,7 @@
 #include <vector>
 
 #include "gemm_tc2.cuh"
+#include "ppo_terms.cuh"
 
 namespace dwbc {
 
@@ -78,30 +79,6 @@ struct alignas(16) C2Prog {
   C2Op op[C2_MAX_OPS];
 };
 static_assert(sizeof(C2Prog) % 16 == 0, "copied to shared memory in 16-byte pieces");
-
-// everything the epilogue hooks need (AC:326-345, PPO:166-221)
-struct FinArgs {
-  const float* std;                                          // [n_act]
-  // FIN_ACT (rollout): a = mu + std * eps.  actions == nullptr: the mean only (dwbc_policy_mean; eps, log_prob, sigma_out unread)
-  const float* eps; float* actions; float* log_prob; float* mean_out; float* sigma_out;
-  // FIN_PPO / FIN_VALUE / FIN_REG (update)
-  const int64_t* idx;                                        // mini-batch gather index (storage row of mini-batch row r)
-  const float* s_actions; const float* old_logp; const float* old_values; const float* returns; const float* adv;
-  const float* zh; int64_t zh_ld; int zh_by_src;
-  float* g_leg; int gleg_ld; float* g_arm; int garm_ld; float* g_v; int gv_ld; float* g_z; int gz_ld;
-  float* grad_std; float* losses;
-  float* part;                                               // [rows / 16][C2_FIN_PART] partial sums, one slot per (tile, worker warp)
-  int n_leg, n_act, latent, rows;
-  float clip, c_value, c_ent, c_reg, rho;
-  int clipped_value;
-  // arm torque supervision (PPO:224-239, fixed gains PPO:318-323); ts_target == nullptr: off.  Rows of [T*N, n_arm] storage tensors,
-  // ts_coef = [3][n_arm] default p gains, d gains, default dof positions; ts_w = schedule weight (PPO:304-305); losses[4] += mean loss
-  const float* ts_target; const float* ts_pos; const float* ts_vel; const float* ts_coef;
-  float ts_w;
-  // optional device (c_reg, rho, ts_w) in place of the three fields (dwbc_ppo_minibatch_grad_sched): chain2_kernel loads them once per CTA into
-  // C2Shared, and the hooks take them from there
-  const float* sched;
-};
 
 struct C2Launch {
   int nprog, x3;             // programs (1 or 2), error-compensated mode
@@ -199,13 +176,6 @@ __device__ __forceinline__ int c2_uni(int v) { return __shfl_sync(0xffffffffu, v
 template <int kRegs> __device__ __forceinline__ void c2_reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs)); }
 template <int kRegs> __device__ __forceinline__ void c2_reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs)); }
 __device__ __forceinline__ void c2_wbar() { __syncwarp(); asm volatile("bar.sync 1, %0;" ::"n"(C2_NW) : "memory"); }     // the worker warps
-constexpr float C2_LOG_SQRT_2PI = 0.91893853320467274178f;
-// One action's term of the Gaussian log-prob (AC:341-345), log_sg = logf(sg).  The PPO loss of both paths (c2_fin_ppo, ppo_loss_kernel) and
-// ppo_diag_kernel sum it over a channel's actions in index order, so the diagnostics see the ratio the loss saw, bit for bit.
-__device__ __forceinline__ float ppo_logp_term(float a, float mu, float sg, float log_sg) {
-  const float d = a - mu;
-  return -(d * d) / (2.0f * (sg * sg)) - log_sg - C2_LOG_SQRT_2PI;
-}
 
 // ---- fp32 pairs ---------------------------------------------------------------------------------------------------------
 // two fp32 values side by side in a 64-bit register, as a 16-byte load delivers them; the arithmetic is element-wise
@@ -310,8 +280,7 @@ __device__ __forceinline__ void c2_fin_act(const FinArgs& f, int c, int64_t m, b
     if (i < cnt) {
       mu[i] = v[i];
       ac[i] = mu[i] + sg[i] * ep[i];
-      const float d = ac[i] - mu[i];
-      lp += -(d * d) / (2.0f * (sg[i] * sg[i])) - logf(sg[i]) - C2_LOG_SQRT_2PI;
+      lp += ppo_logp_term(ac[i], mu[i], sg[i], logf(sg[i]));
     }
   }
   c2_st_group(f.actions + m * f.n_act + off, cnt, vec2, ac);
@@ -319,14 +288,10 @@ __device__ __forceinline__ void c2_fin_act(const FinArgs& f, int c, int64_t m, b
   c2_st_group(f.sigma_out + m * f.n_act + off, cnt, vec2, sg);
   f.log_prob[2 * m + c] = lp;
 }
-// Arm torque supervision (PPO:224-239, off in the shipped config WGC:173) of arm joint i: tau = kp (mu + q_default - q) - kd qd (fixed gains,
-// PPO:318-323) on act_inference(obs)[:, -n_arm:] (PPO:230: the arm means this hook holds), loss = w * mean((tau - target)^2) (PPO:236-238).
-// Returns (squared error, d loss / d pre-tanh output).  Deliberately NOT inlined and scalar-only (no array leaves the caller's registers): the
-// optional branch must not cost the hot epilogue anything.
+// Arm torque supervision of arm joint i on the arm means this hook holds (ppo_torque_term).  Deliberately NOT inlined and scalar-only (no
+// array leaves the caller's registers): the optional branch must not cost the hot epilogue anything.
 __device__ __noinline__ float2 c2_fin_torque(const FinArgs& f, int64_t src, int cnt, int i, float mu, float ts_w) {
-  const float kp = f.ts_coef[i];
-  const float e = kp * (mu + f.ts_coef[2 * cnt + i] - f.ts_pos[src * cnt + i]) - f.ts_coef[cnt + i] * f.ts_vel[src * cnt + i] - f.ts_target[src * cnt + i];
-  return make_float2(e * e, 2.0f * ts_w / ((float)f.rows * (float)cnt) * e * kp * (1.0f - mu * mu));
+  return ppo_torque_term(f, src, cnt, i, mu, ts_w);
 }
 // FIN_PPO (AC:341-345, PPO:199-205): log-prob of the stored action, ratio, mixed advantage, clipped surrogate, entropy and
 // the gradients w.r.t. the mean (through the tanh, AC:157,170) and std of this group
@@ -348,28 +313,18 @@ __device__ __forceinline__ void c2_fin_ppo(const FinArgs& f, int c, int64_t m, b
       if (i < cnt) {
         const float ls = logf(sg[i]);
         lp += ppo_logp_term(act[i], v[i], sg[i], ls);
-        l_ent += 0.5f + C2_LOG_SQRT_2PI + ls;
+        l_ent += ppo_entropy_term(ls);
       }
     }
-    const float mix = c == 0 ? adv.x + rho * adv.y : adv.y + rho * adv.x;          // PPO:199-201
-    const float ratio = expf(lp - old_lp);                                           // PPO:202
-    const float rc = fminf(fmaxf(ratio, 1.0f - f.clip), 1.0f + f.clip);
-    const float s1 = -mix * ratio, s2 = -mix * rc;                                   // PPO:203-205
-    l_surr = fmaxf(s1, s2);
-    const bool inside = ratio >= 1.0f - f.clip && ratio <= 1.0f + f.clip;
-    float g;
-    if (s1 > s2) g = -mix;
-    else if (s1 == s2) g = 0.5f * -mix + (inside ? 0.5f * -mix : 0.0f);
-    else g = inside ? -mix : 0.0f;
-    glp = inv2m * g * ratio;
+    const float ratio = ppo_ratio(lp, old_lp);
+    const float2 surr = ppo_surrogate(ppo_mix(adv, c, rho), ratio, f.clip);
+    l_surr = surr.x;
+    glp = inv2m * surr.y * ratio;
     const int gld = c == 0 ? f.gleg_ld : f.garm_ld;
 #pragma unroll
     for (int i = 0; i < C2_GRP; ++i) {
       gm[i] = 0.0f;
-      if (i < cnt) {
-        const float d = act[i] - v[i];
-        gm[i] = glp * d / (sg[i] * sg[i]) * (1.0f - v[i] * v[i]);
-      }
+      if (i < cnt) gm[i] = ppo_grad_mean(glp, act[i], v[i], sg[i]);
     }
     if (c == 1 && f.ts_target != nullptr) {
 #pragma unroll
@@ -392,10 +347,7 @@ __device__ __forceinline__ void c2_fin_ppo(const FinArgs& f, int c, int64_t m, b
   for (int i = 0; i < C2_GRP; ++i) {           // gradient of std: one warp sum per column
     if (i < cnt) {                             // (warp-uniform)
       float gs = 0.0f;
-      if (on) {
-        const float d = act[i] - v[i];
-        gs = glp * ((d * d) / (sg[i] * sg[i] * sg[i]) - 1.0f / sg[i]) - f.c_ent * inv2m / sg[i];
-      }
+      if (on) gs = ppo_grad_std(glp, act[i], v[i], sg[i], f.c_ent, inv2m);
       gs = warp_sum(gs);
       if (lane == 0) slot[C2P_STD + off + i] = gs;
     }
@@ -413,22 +365,9 @@ __device__ __forceinline__ void c2_fin_value(const FinArgs& f, int c, int64_t m,
   float l_val = 0.0f;
   if (on) {
     const int64_t src = f.idx ? f.idx[m] : m;
-    const float vo = f.old_values[2 * src + c], R = f.returns[2 * src + c];
-    const float l1 = (val - R) * (val - R);
-    float gv;
-    if (f.clipped_value) {
-      const float dvo = val - vo;
-      const float vc = vo + fminf(fmaxf(dvo, -f.clip), f.clip);
-      const float l2 = (vc - R) * (vc - R);
-      const bool inside = dvo >= -f.clip && dvo <= f.clip;
-      l_val = fmaxf(l1, l2);
-      const float g1 = 2.0f * (val - R), g2 = inside ? 2.0f * (vc - R) : 0.0f;
-      gv = l1 > l2 ? g1 : (l1 == l2 ? 0.5f * g1 + 0.5f * g2 : g2);
-    } else {
-      l_val = l1;
-      gv = 2.0f * (val - R);
-    }
-    f.g_v[m * f.gv_ld + c] = gv * f.c_value * inv2m;
+    const float2 t = ppo_value_term(val, f.old_values[2 * src + c], f.returns[2 * src + c], f.clip, f.clipped_value);
+    l_val = t.x;
+    f.g_v[m * f.gv_ld + c] = t.y * f.c_value * inv2m;
     if (c == 0) for (int i = 2; i < f.gv_ld; ++i) f.g_v[m * f.gv_ld + i] = 0.0f;     // pad columns are operand columns of the backward pass
   }
   const float s = warp_sum(l_val * inv2m);
@@ -441,11 +380,8 @@ __device__ __forceinline__ void c2_fin_reg(const FinArgs& f, int64_t m, bool on,
   if (on) {
     const int64_t src = f.idx ? f.idx[m] : m;
     const float* zhr = f.zh + (f.zh_by_src ? src : m) * f.zh_ld;
-#pragma unroll
-    for (int i = 0; i < 32; ++i)
-      if (i < f.latent) { const float d = v[i] - zhr[i]; nrm += d * d; }
-    nrm = sqrtf(nrm);
-    const float s = nrm > 0.0f ? c_reg * invm / nrm : 0.0f;
+    nrm = ppo_reg_norm<32>(v, zhr, f.latent);
+    const float s = ppo_reg_scale(nrm, c_reg, invm);
 #pragma unroll
     for (int i = 0; i < 32; ++i)
       if (i < f.gz_ld) f.g_z[m * f.gz_ld + i] = i < f.latent ? s * (v[i] - zhr[i]) : 0.0f;
