@@ -3,8 +3,9 @@
 rollout (policy forward -> post-physics step -> reward bootstrap) x T, GAE, update(): the same
 sequence `OnPolicyRunner.learn` drives (rsl_rl/rsl_rl/runners/on_policy_runner.py:125-169), on
 synthetic sim-state tensors.  Used only by bench.py (`cpu_baseline` leg and `--impl reference`:
-the reference is pure Python and /root/reference does not exist on the GPU box, so the pinned
-oracle port is what runs there) and by tests.
+the reference is pure Python and may not be installed where the benchmark runs, so the pinned
+oracle port is what runs there).  The tests check the production loop stage by stage instead
+(tests/test_gpu_training_iteration.py), each stage recomputed from the GPU's previous one.
 """
 from __future__ import annotations
 

@@ -178,6 +178,7 @@ def test_transition_written_directly_into_storage_rows():
         alg.init_storage(N, T, [p.num_obs], [None], [p.num_actions])
         alg.storage.values.normal_(generator=torch.Generator(device="cuda").manual_seed(3))
         algs.append(alg)
+    n_timeout = n_done = 0
     for t in range(T):
         sim = synth.sim_state(p, seed, t + 1)
         load_sim(a, p, sim)
@@ -192,7 +193,15 @@ def test_transition_written_directly_into_storage_rows():
         algs[1].process_env_step(b.rew_buf, b.arm_rew_buf, b.reset_buf, b.extras)
         assert n1 - n0 == 1 and int(a._lib.dwbc_launch_count()) == n1          # the second call launched nothing
         assert torch.equal(sa.rewards[t], sb.rewards[t]) and torch.equal(sa.dones[t], sb.dones[t])
-    assert float(algs[0].storage.rewards.abs().sum()) > 0 and int(a.time_out_buf.sum() + sa.dones.sum()) >= 0
+        # the bootstrap changed the rows of the timed-out envs (gamma * values, PPO:133-134) and no other row
+        to, raw = a.time_out_buf, torch.stack([a.rew_buf, a.arm_rew_buf], dim=-1)
+        assert torch.equal(sb.rewards[t][~to], raw[~to])
+        assert bool((sb.rewards[t][to] != raw[to]).all(dim=-1).all())
+        torch.testing.assert_close(sb.rewards[t][to], raw[to] + 0.99 * sb.values[t][to], rtol=1e-6, atol=1e-6)
+        n_timeout += int(to.sum())
+        n_done += int(sb.dones[t].sum())
+    assert float(algs[0].storage.rewards.abs().sum()) > 0
+    assert n_timeout > 0 and n_done > n_timeout, (n_timeout, n_done)          # time-outs and terminations both occurred
 
 
 @pytest.mark.gpu
