@@ -495,10 +495,10 @@ class FusedWidowGo1Core:
             self._stats.zero_()
         return self.extras["episode"]
 
-    def _fill_episode_extras(self):
-        """extras['episode'] (WG:743-750).  One D2H read of the per-step stats block (the reference
-        syncs on len(env_ids) at WG:705 as well)."""
-        st = self._stats.cpu()
+    def _fill_episode_extras(self, st=None, coeffs=None):
+        """extras['episode'] (WG:743-750) from the stats block `st` on the host (default: one D2H read of the device block; the reference
+        syncs on len(env_ids) at WG:705 as well) and the curriculum coefficients `coeffs` (default: the current ones)."""
+        st = self._stats.cpu() if st is None else st
         cnt = float(st[0])
         if cnt > 0:
             ep = {}
@@ -507,12 +507,15 @@ class FusedWidowGo1Core:
             for i, k in enumerate(METRIC_NAMES):
                 ep["metric_" + k] = st[1 + len(self.sum_names) + i] / cnt / self.p.max_episode_length_s
             self.extras["episode"] = ep
-        cur = self.curriculum
-        e = self.extras["episode"]
-        e["coeff_lin_vel_x_upper_bound"], e["coeff_lin_vel_x_lower_bound"] = cur.lin_vel_x_ranges[1], cur.lin_vel_x_ranges[0]
-        e["coeff_ang_vel_yaw_upper_bound"], e["coeff_ang_vel_yaw_lower_bound"] = cur.ang_vel_yaw_ranges[1], cur.ang_vel_yaw_ranges[0]
-        e["coeff_tracking_ang_vel_yaw_exp"] = cur.reward_scales.get("tracking_ang_vel_yaw_exp", 0.0)
+        self.extras["episode"].update(self._curriculum_coeffs() if coeffs is None else coeffs)
         self.reset_count = int(cnt)
+
+    def _curriculum_coeffs(self):
+        """The command-curriculum values _fill_episode_extras adds to extras['episode']."""
+        cur = self.curriculum
+        return dict(coeff_lin_vel_x_upper_bound=cur.lin_vel_x_ranges[1], coeff_lin_vel_x_lower_bound=cur.lin_vel_x_ranges[0],
+                    coeff_ang_vel_yaw_upper_bound=cur.ang_vel_yaw_ranges[1], coeff_ang_vel_yaw_lower_bound=cur.ang_vel_yaw_ranges[0],
+                    coeff_tracking_ang_vel_yaw_exp=cur.reward_scales.get("tracking_ang_vel_yaw_exp", 0.0))
 
     @property
     def sim_state_dirty(self) -> bool:

@@ -23,21 +23,13 @@ from .actor_critic import PolicyMean
 
 
 class HostUpload:
-    """Host values into a device buffer with one asynchronous, stream-ordered copy: the values go through a pinned staging buffer, which
-    is refilled only after the copy that last read it has run (a pageable source would make the copy wait for the whole stream)."""
-
-    def __init__(self):
-        self._pinned, self._done = None, None
+    """Host values into a device buffer with one asynchronous, stream-ordered copy that never waits for the device.  The values go
+    through a fresh pinned staging buffer from PyTorch's caching host allocator, which records the copy and hands the buffer out again
+    only once the copy has run (a pageable source would make the copy wait for the whole stream, and refilling one staging buffer would
+    wait for the copy before).  So a loop can enqueue many iterations ahead of the GPU (GraphRunner)."""
 
     def __call__(self, dst: torch.Tensor, host: torch.Tensor):
-        if self._pinned is None or self._pinned.shape != host.shape or self._pinned.dtype != host.dtype:
-            self._pinned, self._done = torch.empty(host.shape, dtype=host.dtype).pin_memory(), None
-        if self._done is not None:
-            self._done.synchronize()
-        self._pinned.copy_(host)
-        dst.copy_(self._pinned, non_blocking=True)
-        self._done = torch.cuda.Event()
-        self._done.record()
+        dst.copy_(host.pin_memory(), non_blocking=True)
 
 
 # DwbcEnvBuffers fields a captured rollout sets per step itself (observation / transition targets) or re-binds through physics(t)
@@ -46,11 +38,12 @@ _PER_STEP_FIELDS = {"obs_buf", "obs_stride", "store_values", "store_rewards", "s
 
 
 class RolloutGraph:
-    def __init__(self, alg, env, physics=None):
+    def __init__(self, alg, env, physics=None, capture=True):
         """`physics(t)` stands for the simulator of step t.  It runs during capture only: it may re-bind the core's simulator tensors
         (`env.bind_sim`) or enqueue device work, and must not read results on the host.  The simulator tensors it binds are part of the
-        graph: binding other tensors at run time needs a new RolloutGraph."""
-        self.alg, self.env, self.physics = alg, env, physics
+        graph: binding other tensors at run time needs a new RolloutGraph.  `capture=False` issues the same launches eagerly on every
+        run, physics(t) included."""
+        self.alg, self.env, self.physics, self.capture = alg, env, physics, bool(capture)
         self._graphs = {}                        # key() -> CUDAGraph: PPO and DAgger rollouts alternate without re-capturing
         self._record = torch.zeros(C.sizeof(L.StepDevice), dtype=torch.uint8, device=env.device)
         self._upload = HostUpload()
@@ -84,12 +77,6 @@ class RolloutGraph:
 
     def _capture(self, key, hist_encoding):
         alg, env, s = self.alg, self.env, self.alg.storage
-        T, n = s.num_transitions_per_env, s.num_envs
-        na = alg.actor_critic.num_leg_actions + alg.actor_critic.num_arm_actions
-        if alg._eps_all is None or alg._eps_all.shape[:2] != (T, n):
-            alg._eps_all = torch.empty(T, n, na, device=alg.device)
-            alg._eps_valid = False
-        alg._workspace(n)
         self._graphs.pop(key, None)
         counter = env.common_step_counter
         alg._packed = False                          # step 0 of every replay packs the weight images, as the first eager act() does
@@ -113,18 +100,25 @@ class RolloutGraph:
         if s.step != 0:
             raise L.DwbcError("a captured rollout starts at storage row 0")
         alg._set_precision()
-        alg._workspace(s.num_envs)
-        key = self.key(hist_encoding)
-        if key not in self._graphs:
-            self._capture(key, hist_encoding)
+        T, n = s.num_transitions_per_env, s.num_envs
+        alg._workspace(n)
+        na = alg.actor_critic.num_leg_actions + alg.actor_critic.num_arm_actions
+        if alg._eps_all is None or alg._eps_all.shape[:2] != (T, n):
+            alg._eps_all = torch.empty(T, n, na, device=alg.device)
+            alg._eps_valid = False
+        if self.capture:
+            key = self.key(hist_encoding)
+            if key not in self._graphs:
+                self._capture(key, hist_encoding)
         row0 = s.obs_row(0)
         if obs.data_ptr() != row0.data_ptr():
             row0.copy_(obs)
         alg._eps_all.normal_(generator=alg.generator)                                   # FusedPPO.act at t = 0
         alg._eps_valid = True
+        if not self.capture:
+            return self._steps(hist_encoding)
         self._upload(self._record, env.step_record())
         self._graphs[key].replay()
-        T = s.num_transitions_per_env
         s.step = T
         env.common_step_counter += T
         alg._packed, alg._packed_key = True, (s.num_envs, int(bool(hist_encoding)), alg.actor_critic.flat._version)

@@ -29,6 +29,47 @@ from .storage import FusedRolloutStorage
 CHECKPOINT_VERSION = 1          # layout of FusedPPO.state_dict()
 
 
+# The host arithmetic of the readers of FusedPPO (update(), update_dagger(), episode_buffers(), update_diagnostics()), shared with
+# GraphRunner.logs(), which applies it to copies of the same device values taken at the end of each iteration.
+def loss_means(sums, num_updates):
+    """The mean losses of an update from the sums in `_losses` (surrogate, value, priv-reg, entropy, arm torques).  Evaluated where the
+    sums are, on the device in update() and in GraphRunner.logs() alike, so that the two give the same bits."""
+    return sums / num_updates
+
+
+def ppo_result(losses, sched, torque_supervision):
+    """update()'s 7-tuple (PPO:263) from the mean losses (a list) and the schedule values _ppo_end returns."""
+    value_mixing_ratio, ts_w, priv_reg_coef = sched
+    return losses[1], losses[0], (losses[4] if torque_supervision else 0.0), value_mixing_ratio, ts_w, losses[2], priv_reg_coef
+
+
+def dagger_loss(loss_sum, num_updates):
+    """update_dagger()'s mean history-latent loss from the sum in `_losses[0]`."""
+    return float(loss_sum) / num_updates
+
+
+def ring_buffers(ring, pos):
+    """OPR's rewbuffer, arm_rewbuffer and lenbuffer (Python float lists, oldest first) from an episode tracker's ring [C, 3] and
+    position [2] (next slot, episodes appended since tracking began), both on the host."""
+    cap = ring.shape[0]
+    n = min(int(pos[1]), cap)
+    rows = ring[(int(pos[0]) - n + torch.arange(n)) % cap]
+    return dict(rewbuffer=rows[:, 0].tolist(), arm_rewbuffer=rows[:, 1].tolist(), lenbuffer=rows[:, 2].tolist())
+
+
+def diagnostics_from(d, ev):
+    """update_diagnostics()'s dictionary from the per-mini-batch slots d [mini-batches, DIAG_N] and the explained variances ev [2], both
+    on the host."""
+    d = d.double()
+    per = dict(approx_kl=(d[:, L.DIAG_KL_LEG] + d[:, L.DIAG_KL_ARM]).tolist(), approx_kl_leg=d[:, L.DIAG_KL_LEG].tolist(),
+               approx_kl_arm=d[:, L.DIAG_KL_ARM].tolist(), clip_fraction_leg=d[:, L.DIAG_CLIP_LEG].tolist(),
+               clip_fraction_arm=d[:, L.DIAG_CLIP_ARM].tolist(), grad_norm=d[:, L.DIAG_GRAD_NORM].tolist())
+    out = {k: sum(v) / len(v) for k, v in per.items()}
+    out.update(grad_norm_max=max(per["grad_norm"]), explained_variance_leg=float(ev[0]), explained_variance_arm=float(ev[1]),
+               per_minibatch=per)
+    return out
+
+
 class _AdamState:
     """Flat Adam state of one parameter group; `state_dict()` mimics torch.optim.Adam's layout."""
 
@@ -312,10 +353,7 @@ class FusedPPO:
         pos = self._episodes["pos"].to("cpu", non_blocking=True)
         if self.device.type == "cuda":
             torch.cuda.current_stream(self.device).synchronize()
-        cap = self.track_episodes
-        n = min(int(pos[1]), cap)
-        rows = ring[(int(pos[0]) - n + torch.arange(n)) % cap]
-        return dict(rewbuffer=rows[:, 0].tolist(), arm_rewbuffer=rows[:, 1].tolist(), lenbuffer=rows[:, 2].tolist())
+        return ring_buffers(ring, pos)
 
     def _episodes_shape(self):
         return None if self._episodes is None else (self._episodes["running"].shape[0], self.track_episodes)
@@ -349,7 +387,11 @@ class FusedPPO:
 
     # ------------------------------------------------------------------ update (PPO:152-263)
     def update(self, indices=None, on_step=None):
-        if self.cuda_graphs and on_step is None:
+        return self._ppo_finish(self._ppo_run(self.cuda_graphs and on_step is None, indices, on_step))
+
+    def _ppo_run(self, graphed, indices=None, on_step=None):
+        """Every launch of update(), eager or (graphed) as the replay of its CUDA graph; returns the hyper-parameters they ran with."""
+        if graphed:
             return self._update_graphed("ppo", indices)
         ac, s, hp = self.actor_critic, self.storage, self._fill_hp()
         self._set_precision()
@@ -361,7 +403,7 @@ class FusedPPO:
         ws = self._workspace(mbs)
         self._diag_buffer()
         self._ppo_launches(hp, indices, mbs, ws, on_step)
-        return self._ppo_finish(hp)
+        return hp
 
     def _diag_buffer(self):
         """The per-mini-batch diagnostics slots of one update() (diagnostics on), allocated for the current mini-batch count."""
@@ -433,18 +475,21 @@ class FusedPPO:
         s.set_hist_latent(None)
 
     def _ppo_finish(self, hp):
-        s = self.storage
-        num_updates = self.num_learning_epochs * self.num_mini_batches
-        losses = (self._losses / num_updates).tolist()                                   # single sync per update
-        s.clear()
+        losses = loss_means(self._losses, self.num_learning_epochs * self.num_mini_batches).tolist()      # single sync per update
+        sched = self._ppo_end(hp)
+        self.last_entropy = losses[3]
+        return ppo_result(losses, sched, self.torque_supervision)
+
+    def _ppo_end(self, hp):
+        """What _ppo_finish does besides reading the losses, which stay in `_losses` on the device: clear the storage, advance
+        `counter`, enforce_min_std().  Returns the host-side schedule values of update()'s 7-tuple (ppo_result's `sched`)."""
+        self.storage.clear()
         if self.diagnostics:
-            self._diag_steps = num_updates
-        value_mixing_ratio, priv_reg_coef = hp.mixing_ratio, hp.priv_reg_coef
+            self._diag_steps = self.num_learning_epochs * self.num_mini_batches
         self.counter += 1                                                                 # PPO:259
         self.enforce_min_std()
-        self.last_entropy = losses[3]
-        ts_w = hp.torque_supervision_weight if self.torque_supervision else 0                            # PPO:158
-        return losses[1], losses[0], (losses[4] if self.torque_supervision else 0.0), value_mixing_ratio, ts_w, losses[2], priv_reg_coef  # PPO:263
+        ts_w = hp.torque_supervision_weight if self.torque_supervision else 0            # PPO:158
+        return hp.mixing_ratio, ts_w, hp.priv_reg_coef
 
     def update_diagnostics(self):
         """Diagnostics of the last update() (FusedPPO(diagnostics=True)), read with one synchronisation: the means over its mini-batches
@@ -461,19 +506,18 @@ class FusedPPO:
         ev = self._diag_ev.to("cpu", non_blocking=True)
         if self.device.type == "cuda":
             torch.cuda.current_stream(self.device).synchronize()
-        d = d.double()
-        per = dict(approx_kl=(d[:, L.DIAG_KL_LEG] + d[:, L.DIAG_KL_ARM]).tolist(), approx_kl_leg=d[:, L.DIAG_KL_LEG].tolist(),
-                   approx_kl_arm=d[:, L.DIAG_KL_ARM].tolist(), clip_fraction_leg=d[:, L.DIAG_CLIP_LEG].tolist(),
-                   clip_fraction_arm=d[:, L.DIAG_CLIP_ARM].tolist(), grad_norm=d[:, L.DIAG_GRAD_NORM].tolist())
-        out = {k: sum(v) / len(v) for k, v in per.items()}
-        out.update(grad_norm_max=max(per["grad_norm"]), explained_variance_leg=float(ev[0]), explained_variance_arm=float(ev[1]),
-                   per_minibatch=per)
-        return out
+        return diagnostics_from(d, ev)
 
     def update_dagger(self, indices=None):
         """PPO:265-291."""
-        if self.cuda_graphs:
-            return self._update_graphed("dagger", indices)
+        self._dagger_run(self.cuda_graphs, indices)
+        return self._dagger_finish()
+
+    def _dagger_run(self, graphed, indices=None):
+        """Every launch of update_dagger(), eager or (graphed) as the replay of its CUDA graph."""
+        if graphed:
+            self._update_graphed("dagger", indices)
+            return
         s, hp = self.storage, self._fill_hp()
         self._set_precision()
         self._packed = False
@@ -483,7 +527,6 @@ class FusedPPO:
         mbs = indices.numel() // self.num_mini_batches
         ws = self._workspace(mbs)
         self._dagger_launches(hp, indices, mbs, ws)
-        return self._dagger_finish()
 
     def _dagger_launches(self, hp, indices, mbs, ws, dev=None):
         """Every launch of one update_dagger(); dev as in _ppo_launches (only its Adam table is read)."""
@@ -506,11 +549,14 @@ class FusedPPO:
                         "dwbc_clip_adam_step_table")
 
     def _dagger_finish(self):
-        num_updates = self.num_learning_epochs * self.num_mini_batches
-        loss = float(self._losses[0]) / num_updates
+        loss = dagger_loss(self._losses[0], self.num_learning_epochs * self.num_mini_batches)
+        self._dagger_end()
+        return loss
+
+    def _dagger_end(self):
+        """What _dagger_finish does besides reading the loss, which stays in `_losses[0]` on the device."""
         self.storage.clear()
         self.counter += 1
-        return loss
 
     # ------------------------------------------------------------------ CUDA graphs of update() / update_dagger()
     def graph_key(self, kind):
@@ -556,7 +602,7 @@ class FusedPPO:
         g["upload"](g["scalars"], host)
         g["graph"].replay()
         opt.step += n_steps
-        return self._ppo_finish(hp) if kind == "ppo" else self._dagger_finish()
+        return hp
 
     def _capture(self, kind, key, mbs, n_idx, n_steps):
         self._graphs.pop(kind, None)
