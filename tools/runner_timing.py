@@ -14,7 +14,15 @@ in a synchronise).  A separate phase then profiles one block of each arm with to
 from the first to the last GPU activity minus the union of the kernel / memcpy / memset intervals, per iteration, and the largest gap.
 All arms must end with bitwise-equal parameters.  The card's name, power limit and clocks are read in the same run.
 
+With --eval-interval, the cost of scheduled evaluation and of the timing events instead: two arms of GraphRunner(capture=True,
+log_interval=--block) on the same workload, both evaluating the teacher and the student (--eval-steps steps) every --eval-interval
+iterations on a second core (bench.py's workload of rank 1), one with timing=True's events and one without, alternating blocks as above.
+Reported: the iteration time of each arm, the rows' GPU times (collection, learning, evaluation per evaluated iteration), the GPU time
+of one mode's evaluation alone (CUDA events around the snapshot restore and the EvalGraph replay, per mode), and the host time that
+enqueueing an evaluation adds to an evaluated iteration.  Both arms must end with bitwise-equal parameters.
+
     python tools/runner_timing.py [--block 20] [--reps 7] [--warmup 1] [--out DIR]
+    python tools/runner_timing.py --eval-interval 10 --eval-steps 1000 [--block 20] [--reps 7] [--warmup 1] [--out DIR]
 """
 import argparse
 import json
@@ -84,6 +92,90 @@ def block(arm, w, n):
     return rows
 
 
+def build_eval(timing, args):
+    """bench.py's workload under a GraphRunner that evaluates on the core of a second workload (rank 1)."""
+    import bench
+    from dwbc_b200 import ppo
+    from dwbc_b200.runner import GraphRunner
+    orig = ppo.FusedPPO
+
+    class Tracking(orig):
+        def __init__(self, *a, **k):
+            super().__init__(*a, track_episodes=100, **k)
+    ppo.FusedPPO = Tracking
+    try:
+        w = bench.Workload("cuda:0", 0, precision="tf32x3")
+        ev = bench.Workload("cuda:0", 1, precision="tf32x3")
+    finally:
+        ppo.FusedPPO = orig
+    w.ev = ev
+    w.runner = GraphRunner(w.alg, w.env, lambda t: w.env.bind_sim(**w.pool[t]), log_interval=args.block, capture=True, eval_env=ev.env,
+                           eval_interval=args.eval_interval, eval_steps=args.eval_steps,
+                           eval_physics=lambda t: ev.env.bind_sim(**ev.pool[t % len(ev.pool)]), timing=timing)
+    w.enqueue = []                                      # host seconds spent enqueueing each evaluation
+    evaluate = w.runner._evaluate
+
+    def timed():
+        t0 = time.perf_counter()
+        evaluate()
+        w.enqueue.append(time.perf_counter() - t0)
+    w.runner._evaluate = timed
+    return w
+
+
+def eval_main(args, info):
+    arms = ("timing_off", "timing_on")
+    work = {arm: build_eval(arm == "timing_on", args) for arm in arms}
+    for _ in range(args.warmup):
+        for arm in arms:
+            work[arm].runner.learn(args.block)
+            work[arm].runner.logs()
+    res, rows = {arm: [] for arm in arms}, []
+    for arm in arms:
+        work[arm].enqueue.clear()
+    for _ in range(args.reps):
+        for arm in arms:
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            work[arm].runner.learn(args.block)
+            torch.cuda.synchronize()
+            res[arm].append(1e3 * (time.perf_counter() - t0) / args.block)
+            out = work[arm].runner.logs()
+            if arm == "timing_on":
+                rows += out
+    med = lambda v: dict(median=statistics.median(v), min=min(v), max=max(v), n=len(v))  # noqa: E731
+    r = work["timing_on"].runner
+    per_mode = {}
+    for m, g in r._evals.items():                       # one mode alone: restore + replay, between CUDA events
+        times = []
+        for _ in range(args.reps):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            r.eval_env.load_state_dict(r._eval_start)
+            for v in g._episodes.values():
+                v.zero_()
+            g.run(r.eval_env.obs_buf)
+            e1.record()
+            e1.synchronize()
+            times.append(e0.elapsed_time(e1))
+        per_mode[m] = med(times)
+    evaluated = [row for row in rows if "eval_time" in row]
+    out = dict(gpu=info, block=args.block, reps=args.reps, warmup=args.warmup, eval_interval=args.eval_interval, eval_steps=args.eval_steps,
+               iteration_ms={arm: med(v) for arm, v in res.items()},
+               rows=dict(collection_ms=med([1e3 * x["collection_time"] for x in rows]), learn_ms=med([1e3 * x["learn_time"] for x in rows]),
+                         fps=med([x["fps"] for x in rows]), eval_ms=med([1e3 * x["eval_time"] for x in evaluated]),
+                         captured_rows=sum(x["captured"] for x in rows)),
+               eval_mode_ms=per_mode, eval_enqueue_host_ms={arm: med([1e3 * t for t in work[arm].enqueue]) for arm in arms},
+               last_eval={m: {k: v for k, v in e.items() if k != "episode"} for m, e in evaluated[-1]["eval"].items()},
+               parameters_equal=bool(torch.equal(work["timing_off"].alg.actor_critic.flat, work["timing_on"].alg.actor_critic.flat)))
+    print(json.dumps(out, indent=1))
+    if args.out:
+        os.makedirs(args.out, exist_ok=True)
+        with open(os.path.join(args.out, "runner_eval_timing.json"), "w") as f:
+            json.dump(out, f, indent=1)
+    assert out["parameters_equal"]
+
+
 def gpu_idle(prof, n):
     """GPU idle time (ms per iteration) over the profiled block and the largest single gap (ms)."""
     spans = sorted((e.time_range.start, e.time_range.end) for e in prof.events()
@@ -109,10 +201,14 @@ def main():
     ap.add_argument("--reps", type=int, default=7)
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--eval-interval", type=int, default=None, help="measure scheduled evaluation every this many iterations instead")
+    ap.add_argument("--eval-steps", type=int, default=1000)
     args = ap.parse_args()
     assert torch.cuda.is_available(), "runner_timing.py measures on a CUDA device"
     from graph_timing import gpu_info
     info = gpu_info()
+    if args.eval_interval is not None:
+        return eval_main(args, info)
     work = {arm: build(arm) for arm in ARMS}
     for _ in range(args.warmup):
         for arm in ARMS:
